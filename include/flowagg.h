@@ -231,7 +231,9 @@ enum fa_mode {
                                LookupAndDeleteMap, merged with the feature folds when FA_F_ENABLE_RTT / FA_F_ENABLE_DNS are
                                set (a flow first seen through a feature sample gets its base from the first packet that
                                follows; such entries count towards max_entries, unlike in the reference where the
-                               feature maps are separate).  FA_F_ENABLE_SKETCH / FA_F_NO_FULL_CUT are refused. */
+                               feature maps are separate).  FA_F_ENABLE_SKETCH / FA_F_NO_FULL_CUT are refused.  With
+                               FA_F_NONBLOCKING_EVICT, fa_ingest* goes on while fa_evict scans the retired map, as
+                               flow_monitor goes on while the evictor runs LookupAndDeleteMap. */
 };
 
 typedef struct fa_config {
@@ -258,8 +260,15 @@ typedef struct fa_config {
 #define FA_F_NONBLOCKING_EVICT 0x40u /* keep a second, empty flow table: fa_evict swaps the two under the engine lock — the
                                      Accounter hands its map over and goes on with a fresh one, pkg/flow/account.go:67-68,
                                      86-87 — and scans the retired table on its own stream, so fa_ingest (another thread)
-                                     never waits for the scan or the copy to the host.  Twice the table memory;
-                                     ACCOUNTER mode without feature folds */
+                                     never waits for the scan or the copy to the host.  ACCOUNTER mode without feature
+                                     folds, or KERNEL_MAP mode with any of FA_F_ENABLE_RTT / FA_F_ENABLE_DNS /
+                                     FA_F_ENABLE_PKT_DROP / FA_F_RINGBUF_FALLBACK (the map and its feature lines are
+                                     swapped together; the DNS correlation table, the fallback ring and the counters are
+                                     not, and max_entries counts against the new map only, as after LookupAndDeleteMap).
+                                     The swapped memory doubles: KERNEL_MAP with all three feature folds keeps 560 B per
+                                     slot, about 2 x 9.4 GB at 2^24 slots.  Flows keep arriving while fa_evict runs, so its
+                                     `cap` must cover max_entries (plus, with feature folds, the flows first seen through
+                                     a feature sample), not the live count read before the call */
 #define FA_F_RINGBUF_FALLBACK 0x10u /* KERNEL_MAP mode: ENABLE_FLOWS_RINGBUF_FALLBACK (config.go:286-288): packets whose flow
                                      cannot be created because the map is full are kept as single-packet records
                                      (errno = E2BIG, bpf/flows.c:262-279) and read back with fa_read_spilled(); without

@@ -55,8 +55,9 @@ constexpr int      TAG_EPOCH_SHIFT = 24;   // 40-bit launch counter
 
 struct Table {
     uint4*   ident;      // slots x 8 uint4
-    uint4*   hot;        // slots x 2 uint4
-    uint4*   feat_add;   // slots x 5 uint4 (80 B) or nullptr: additional_metrics fold state
+    uint4*   hot;        // slots x 2 uint4 (ACCOUNTER mode), or nullptr
+    uint8_t* met;        // slots x 128 B flow_metrics lines (KERNEL_MAP mode, kmap_body.cuh), or nullptr
+    uint4*   feat_add;  // slots x 5 uint4 (80 B) or nullptr: additional_metrics fold state
     uint4*   feat_dns;   // slots x 8 uint4 (128 B) or nullptr: dns_metrics fold state
     uint4*   feat_drop;  // slots x 6 uint4 (96 B) or nullptr: pkt_drop_metrics fold state
     uint32_t* occ;       // occupancy bitmap, 1 bit per slot: eviction visits live flows only

@@ -112,7 +112,8 @@ struct fa_engine {
     fa::Table table{};
     uint64_t slots = 0, epoch = 0;
     // FA_F_NONBLOCKING_EVICT: a second, empty table.  fa_evict swaps the two under `mu` (the Accounter hands its map
-    // over and goes on with a fresh one, pkg/flow/account.go:67-68,86-87) and scans the retired one on its own stream.
+    // over and goes on with a fresh one, pkg/flow/account.go:67-68,86-87; in KERNEL_MAP mode a packet racing
+    // LookupAndDeleteMap lands in a fresh entry) and scans the retired one on its own stream.
     fa::Table table_spare{};
     bool double_buffered = false;
     std::mutex evict_mu;                      // one eviction at a time (the reference's evictor is single-flight)
@@ -166,8 +167,7 @@ struct fa_engine {
     uint32_t ring_n[kLiveRing] = {};
     uint32_t ring_head = 0, ring_tail = 0;       // monotonically increasing; slot = idx % kLiveRing
 
-    // KERNEL_MAP mode (kmap.cu): metrics lines, per-batch scratch, fallback ring
-    uint8_t* km_met = nullptr;
+    // KERNEL_MAP mode (kmap.cu): per-batch scratch, fallback ring (the metric lines are table.met)
     uint32_t* km_slot_of = nullptr;
     fa::KmBEntry* km_bset = nullptr; uint32_t km_bset_slots = 0;
     uint32_t* km_blist = nullptr;
@@ -338,7 +338,7 @@ int ingest_chunk_kmap(fa_engine* e, const uint8_t* d_recs, uint32_t n, uint32_t*
     fa::KmParams P{};
     P.recs = d_recs; P.n = n;
     P.ringbuf = (e->cfg.flags & FA_F_RINGBUF_FALLBACK) ? 1 : 0;
-    P.t = e->table; P.met = e->km_met;
+    P.t = e->table; P.met = e->table.met;
     P.epoch = ++e->epoch;
     P.slot_of = e->km_slot_of;
     P.live = &e->d_ctr->live;
@@ -442,6 +442,32 @@ static uint64_t e_max_batch_tmp(const fa_config* cfg) {
     return mb > (1ull << 28) ? (1ull << 28) : mb;
 }
 
+// Everything fa_evict swaps (FA_F_NONBLOCKING_EVICT): identity lines, occupancy bitmap, the mode's metric lines (hot
+// lines / KERNEL_MAP flow_metrics lines) and the enabled feature lines — zeroed on the engine stream.
+static int alloc_table(fa_engine* e, fa::Table* t) {
+    const uint64_t slots = e->slots;
+    const uint32_t f = e->cfg.flags;
+    auto zeroed = [e](auto** p, size_t bytes) -> int {
+        CU(cudaMalloc(p, bytes));
+        CU(cudaMemsetAsync(*p, 0, bytes, e->stream));
+        return FA_OK;
+    };
+    t->mask = slots - 1;
+    if (int rc = zeroed(&t->ident, slots * fa::kIdentBytes)) return rc;
+    if (int rc = e->cfg.mode == FA_MODE_KERNEL_MAP ? zeroed(&t->met, slots * fa::kMetLineBytes) : zeroed(&t->hot, slots * fa::kHotBytes)) return rc;
+    if (int rc = zeroed(&t->occ, slots / 8)) return rc;
+    if (f & FA_F_ENABLE_RTT) { if (int rc = zeroed(&t->feat_add, slots * 80)) return rc; }
+    if (f & FA_F_ENABLE_DNS) { if (int rc = zeroed(&t->feat_dns, slots * 128)) return rc; }
+    if (f & FA_F_ENABLE_PKT_DROP) { if (int rc = zeroed(&t->feat_drop, slots * 96)) return rc; }
+    return FA_OK;
+}
+
+static void free_table(fa::Table* t) {
+    cudaFree(t->ident); cudaFree(t->hot); cudaFree(t->met); cudaFree(t->occ);
+    cudaFree(t->feat_add); cudaFree(t->feat_dns); cudaFree(t->feat_drop);
+    *t = fa::Table{};
+}
+
 extern "C" {
 
 uint32_t fa_abi_version(void) { return FA_ABI_VERSION; }
@@ -488,16 +514,21 @@ int fa_create(const fa_config* cfg, fa_engine** out) {
     uint64_t want = (4 * cfg->max_entries + 2) / 3;          // 0.75 x 2^k entries get exactly 2^k slots
     uint64_t slots = 1024; while (slots < want) slots <<= 1;
     e->slots = slots;
-    e->table.mask = slots - 1;
-    CU(cudaMalloc(&e->table.ident, slots * fa::kIdentBytes));
-    CU(cudaMemsetAsync(e->table.ident, 0, slots * fa::kIdentBytes, e->stream));
-    if (!kmap) {
-        CU(cudaMalloc(&e->table.hot, slots * fa::kHotBytes));
-        CU(cudaMemsetAsync(e->table.hot, 0, slots * fa::kHotBytes, e->stream));
-    } else {
-        if (slots > (1ull << 30)) return fail(FA_E_INVAL, "fa_create: KERNEL_MAP mode supports at most 2^30 slots");
-        CU(cudaMalloc(&e->km_met, slots * fa::kMetLineBytes));
-        CU(cudaMemsetAsync(e->km_met, 0, slots * fa::kMetLineBytes, e->stream));
+    if (kmap && slots > (1ull << 30)) return fail(FA_E_INVAL, "fa_create: KERNEL_MAP mode supports at most 2^30 slots");
+    const uint32_t feat_flags = FA_F_ENABLE_RTT | FA_F_ENABLE_DNS | FA_F_ENABLE_PKT_DROP;
+    if ((cfg->flags & FA_F_NONBLOCKING_EVICT) && !kmap && (cfg->flags & feat_flags))
+        return fail(FA_E_INVAL, "fa_create: FA_F_NONBLOCKING_EVICT with feature folds needs mode KERNEL_MAP");
+    if (int rc = alloc_table(e, &e->table)) return rc;
+    if (cfg->flags & FA_F_NONBLOCKING_EVICT) {
+        if (int rc = alloc_table(e, &e->table_spare)) return rc;
+        CU(cudaStreamCreateWithFlags(&e->evict_stream, cudaStreamNonBlocking));
+        CU(cudaEventCreateWithFlags(&e->ev_swap, cudaEventDisableTiming));
+        CU(cudaMalloc(&e->d_ctr_ev, sizeof(fa::Counters)));
+        CU(cudaMemsetAsync(e->d_ctr_ev, 0, sizeof(fa::Counters), e->stream));
+        CU(cudaHostAlloc(&e->h_ev_out, 8, cudaHostAllocDefault));
+        e->double_buffered = true;
+    }
+    if (kmap) {
         CU(cudaMalloc(&e->km_slot_of, e->max_batch * 4));
         uint32_t bs = 1024; while ((uint64_t)bs < 2 * e->max_batch) bs <<= 1;
         e->km_bset_slots = bs;
@@ -517,38 +548,7 @@ int fa_create(const fa_config* cfg, fa_engine** out) {
         CU(cudaHostAlloc(&e->h_km_ctr, sizeof(fa::KmCounters), cudaHostAllocDefault));
         memset(e->h_km_ctr, 0, sizeof(fa::KmCounters));
     }
-    CU(cudaMalloc(&e->table.occ, slots / 8));
-    CU(cudaMemsetAsync(e->table.occ, 0, slots / 8, e->stream));
-    if (cfg->flags & FA_F_NONBLOCKING_EVICT) {
-        if (kmap || (cfg->flags & (FA_F_ENABLE_RTT | FA_F_ENABLE_DNS | FA_F_ENABLE_PKT_DROP)))
-            return fail(FA_E_INVAL, "fa_create: FA_F_NONBLOCKING_EVICT is available in ACCOUNTER mode without feature folds");
-        e->table_spare.mask = slots - 1;
-        CU(cudaMalloc(&e->table_spare.ident, slots * fa::kIdentBytes));
-        CU(cudaMemsetAsync(e->table_spare.ident, 0, slots * fa::kIdentBytes, e->stream));
-        CU(cudaMalloc(&e->table_spare.hot, slots * fa::kHotBytes));
-        CU(cudaMemsetAsync(e->table_spare.hot, 0, slots * fa::kHotBytes, e->stream));
-        CU(cudaMalloc(&e->table_spare.occ, slots / 8));
-        CU(cudaMemsetAsync(e->table_spare.occ, 0, slots / 8, e->stream));
-        CU(cudaStreamCreateWithFlags(&e->evict_stream, cudaStreamNonBlocking));
-        CU(cudaEventCreateWithFlags(&e->ev_swap, cudaEventDisableTiming));
-        CU(cudaMalloc(&e->d_ctr_ev, sizeof(fa::Counters)));
-        CU(cudaMemsetAsync(e->d_ctr_ev, 0, sizeof(fa::Counters), e->stream));
-        CU(cudaHostAlloc(&e->h_ev_out, 8, cudaHostAllocDefault));
-        e->double_buffered = true;
-    }
-    if (cfg->flags & FA_F_ENABLE_RTT) {
-        CU(cudaMalloc(&e->table.feat_add, slots * 80));
-        CU(cudaMemsetAsync(e->table.feat_add, 0, slots * 80, e->stream));
-    }
-    if (cfg->flags & FA_F_ENABLE_DNS) {
-        CU(cudaMalloc(&e->table.feat_dns, slots * 128));
-        CU(cudaMemsetAsync(e->table.feat_dns, 0, slots * 128, e->stream));
-    }
-    if (cfg->flags & FA_F_ENABLE_PKT_DROP) {
-        CU(cudaMalloc(&e->table.feat_drop, slots * 96));
-        CU(cudaMemsetAsync(e->table.feat_drop, 0, slots * 96, e->stream));
-    }
-    if (cfg->flags & (FA_F_ENABLE_RTT | FA_F_ENABLE_DNS | FA_F_ENABLE_PKT_DROP)) CU(cudaMalloc(&e->d_slot_of, e_max_batch_tmp(cfg) * 4));
+    if (cfg->flags & feat_flags) CU(cudaMalloc(&e->d_slot_of, e_max_batch_tmp(cfg) * 4));
     CU(cudaMalloc(&e->d_ctr, sizeof(fa::Counters)));
     CU(cudaMemsetAsync(e->d_ctr, 0, sizeof(fa::Counters), e->stream));
     CU(cudaHostAlloc(&e->h_ctr, sizeof(fa::Counters), cudaHostAllocDefault));
@@ -623,11 +623,12 @@ void fa_destroy(fa_engine* e) {
         cudaFree(e->d_prof);
     }
     if (e->copy_stream) { cudaStreamSynchronize(e->copy_stream); cudaStreamDestroy(e->copy_stream); }
+    { std::lock_guard<std::mutex> elk(e->evict_mu); }      // an fa_evict still scanning a retired table returns first
     if (e->evict_stream) { cudaStreamSynchronize(e->evict_stream); cudaStreamDestroy(e->evict_stream); }
     if (e->ev_swap) cudaEventDestroy(e->ev_swap);
-    cudaFree(e->table_spare.ident); cudaFree(e->table_spare.hot); cudaFree(e->table_spare.occ); cudaFree(e->d_ctr_ev);
+    free_table(&e->table_spare); cudaFree(e->d_ctr_ev);
     if (e->h_ev_out) cudaFreeHost(e->h_ev_out);
-    cudaFree(e->table.ident); cudaFree(e->table.hot); cudaFree(e->table.occ); cudaFree(e->table.feat_add); cudaFree(e->table.feat_dns); cudaFree(e->table.feat_drop);
+    free_table(&e->table);
     cudaFree(e->d_ctr); if (e->h_ctr) cudaFreeHost(e->h_ctr);
     if (e->h_live_ring) cudaFreeHost(e->h_live_ring);
     for (int i = 0; i < fa_engine::kLiveRing; i++) if (e->ev_live[i]) cudaEventDestroy(e->ev_live[i]);
@@ -645,7 +646,7 @@ void fa_destroy(fa_engine* e) {
     cudaFree(e->sk.cms); cudaFree(e->sk.hll);
     cudaFree(e->dnsc.tab); cudaFree(e->dnsc_spare); cudaFree(e->dnsc.ctr); cudaFreeHost(e->h_dnsc_ctr);
     cudaFree(e->d_dnsc_state); cudaFree(e->d_dnsc_samples); cudaFree(e->d_dnsc_out); cudaFree(e->d_dnsc_warps);
-    cudaFree(e->km_met); cudaFree(e->km_slot_of); cudaFree(e->km_bset); cudaFree(e->km_blist); cudaFree(e->km_spill);
+    cudaFree(e->km_slot_of); cudaFree(e->km_bset); cudaFree(e->km_blist); cudaFree(e->km_spill);
     cudaFree(e->km_touched); cudaFree(e->km_deferred); cudaFree(e->km_brec);
     cudaFree(e->d_km_ctr); if (e->h_km_ctr) cudaFreeHost(e->h_km_ctr);
     cudaFree(e->d_pb_sizes); cudaFree(e->d_pb_offsets); cudaFree(e->d_pb_sums); cudaFree(e->d_pb_ifaces);
@@ -876,8 +877,72 @@ int fa_live_flows(fa_engine* e, size_t* n) {
     return FA_OK;
 }
 
-// FA_F_NONBLOCKING_EVICT: swap the tables under `mu` (fa_ingest goes on at once, into the empty one), then lookup-and-
-// delete the retired table on the eviction stream.  Only the K1 launches already queued are waited for.
+// Device staging of the host-bound blocks of fa_evict_ex and the slot list of the feature pass, grown on demand.  Only
+// eviction touches it (the blocking path under `mu`, evict_swapped under `evict_mu` alone), never fa_ingest*.
+static int evict_staging(fa_engine* e, uint64_t live, bool records, bool feats) {
+    const uint64_t want = std::max<uint64_t>(live, std::min<uint64_t>(e->cfg.max_entries, live * 2));
+    if (records && e->evict_cap < live) {
+        cudaFree(e->d_evict); e->d_evict = nullptr; e->evict_cap = 0;
+        CU(cudaMalloc(&e->d_evict, want * fa::kRecBytes));
+        e->evict_cap = want;
+    }
+    if (feats && e->feat_evict_cap < live) {
+        cudaFree(e->d_evict_dns); cudaFree(e->d_evict_add); cudaFree(e->d_evict_present); cudaFree(e->d_slot_of_out);
+        cudaFree(e->d_evict_drop); cudaFree(e->d_evict_rttmin);
+        e->d_evict_dns = e->d_evict_add = e->d_evict_present = e->d_evict_drop = nullptr; e->d_evict_rttmin = nullptr;
+        e->d_slot_of_out = nullptr; e->feat_evict_cap = 0;
+        CU(cudaMalloc(&e->d_evict_dns, want * 64)); CU(cudaMalloc(&e->d_evict_add, want * 32));
+        CU(cudaMalloc(&e->d_evict_drop, want * 32)); CU(cudaMalloc(&e->d_evict_rttmin, want * 8));
+        CU(cudaMalloc(&e->d_evict_present, want)); CU(cudaMalloc(&e->d_slot_of_out, want * 4));
+        e->feat_evict_cap = want;
+    }
+    return FA_OK;
+}
+
+// Lookup-and-delete the `live` flows of `t` into the blocks of `o`, on stream `st`: the table scan (K2, or the
+// KERNEL_MAP scan) with ctr->evict_out as its cursor, the feature pass when `t` has feature lines, then the copies of
+// the blocks that are host memory (device blocks are written in place; staging from evict_staging).  The feature
+// blocks of a table without feature lines are not written.  Adds the kernels launched and the bytes copied.
+static int evict_scan(fa_engine* e, const fa::Table& t, const fa_evict_out* o, uint64_t live, fa::Counters* ctr,
+                      cudaStream_t st, uint64_t* launches, uint64_t* d2h) {
+    const bool feats = t.feat_add || t.feat_dns || t.feat_drop;
+    auto dev = [](void* p, void* staging) -> uint8_t* {          // where the kernels write a block
+        return static_cast<uint8_t*>(p && classify(p) != PTR_DEVICE ? staging : p);
+    };
+    uint8_t* d_out = dev(o->records, e->d_evict);
+    uint8_t *d_dns = nullptr, *d_add = nullptr, *d_drop = nullptr, *d_rmin = nullptr, *d_pres = nullptr;
+    if (feats) {
+        d_dns = dev(o->dns, e->d_evict_dns); d_add = dev(o->additional, e->d_evict_add); d_drop = dev(o->pkt_drops, e->d_evict_drop);
+        d_rmin = dev(o->rtt_min, e->d_evict_rttmin); d_pres = dev(o->present, e->d_evict_present);
+        // the block of a feature this engine does not fold comes out zero (the feature pass does not write it)
+        if (d_dns && !t.feat_dns) CU(cudaMemsetAsync(d_dns, 0, live * 64, st));
+        if (d_add && !t.feat_add) CU(cudaMemsetAsync(d_add, 0, live * 32, st));
+        if (d_drop && !t.feat_drop) CU(cudaMemsetAsync(d_drop, 0, live * 32, st));
+    }
+    uint32_t* slot_of_out = feats ? e->d_slot_of_out : nullptr;
+    if (e->cfg.mode == FA_MODE_KERNEL_MAP)
+        *launches += fa::launch_kmap_evict(t, t.met, d_out, live, &ctr->evict_out, slot_of_out, e->sm_count, st);
+    else
+        *launches += fa::launch_evict(t, reinterpret_cast<uint4*>(d_out), slot_of_out, live, ctr, e->sm_count, st);
+    if (feats)
+        *launches += fa::launch_evict_features(t, slot_of_out, live, d_out, d_dns, d_add, d_drop,
+                                               reinterpret_cast<unsigned long long*>(d_rmin), d_pres, e->sm_count, st);
+    CU(cudaGetLastError());
+    const struct { void* host; const uint8_t* src; size_t width; } blocks[6] = {
+        {o->records, d_out, fa::kRecBytes}, {o->dns, d_dns, 64}, {o->additional, d_add, 32}, {o->pkt_drops, d_drop, 32},
+        {o->rtt_min, d_rmin, 8}, {o->present, d_pres, 1}};
+    for (const auto& b : blocks) {
+        if (!b.host || !b.src || b.src == b.host) continue;        // not asked for, not produced, or written in place
+        CU(cudaMemcpyAsync(b.host, b.src, live * b.width, cudaMemcpyDeviceToHost, st));
+        *d2h += live * b.width;
+    }
+    return FA_OK;
+}
+
+// FA_F_NONBLOCKING_EVICT: swap the tables under `mu` (fa_ingest* goes on at once, into the empty one), then lookup-and-
+// delete the retired table on the eviction stream: the scan, the feature pass and the copies to the host.  Only the
+// launches already queued are waited for.  Not swapped: the DNS correlation table, the fallback ring, the KERNEL_MAP
+// counters.
 static int evict_swapped(fa_engine* e, const fa_evict_out* o, size_t cap, size_t* n_out) {
     std::lock_guard<std::mutex> elk(e->evict_mu);
     CU(cudaSetDevice(e->device));
@@ -900,28 +965,19 @@ static int evict_swapped(fa_engine* e, const fa_evict_out* o, size_t cap, size_t
         e->live_known = 0; e->unsynced_records = 0; e->ring_head = e->ring_tail;
         e->st.flows_evicted += live;
     }
-    // from here on fa_ingest runs concurrently
+    // from here on fa_ingest* runs concurrently, into the new table; this side has its own stream, cursor and staging
+    const bool feats = retired.feat_add || retired.feat_dns || retired.feat_drop;
     const PtrKind k = classify(o->records);
-    uint8_t* d_out = static_cast<uint8_t*>(o->records);
-    if (k != PTR_DEVICE) {
-        if (e->evict_cap < live) {
-            cudaFree(e->d_evict); e->d_evict = nullptr; e->evict_cap = 0;
-            uint64_t want = std::max<uint64_t>(live, std::min<uint64_t>(e->cfg.max_entries, live * 2));
-            CU(cudaMalloc(&e->d_evict, want * fa::kRecBytes));
-            e->evict_cap = want;
-        }
-        d_out = e->d_evict;
-    }
+    if (int rc = evict_staging(e, live, k != PTR_DEVICE, feats)) return rc;
     CU(cudaStreamWaitEvent(e->evict_stream, e->ev_swap, 0));
     CU(cudaMemsetAsync(&e->d_ctr_ev->evict_out, 0, sizeof(unsigned long long), e->evict_stream));
-    const int launched = fa::launch_evict(retired, reinterpret_cast<uint4*>(d_out), nullptr, live, e->d_ctr_ev, e->sm_count, e->evict_stream);
-    CU(cudaGetLastError());
-    if (k != PTR_DEVICE) CU(cudaMemcpyAsync(o->records, d_out, live * fa::kRecBytes, cudaMemcpyDeviceToHost, e->evict_stream));
+    uint64_t launched = 0, d2h = 0;
+    if (int rc = evict_scan(e, retired, o, live, e->d_ctr_ev, e->evict_stream, &launched, &d2h)) return rc;
     CU(cudaMemcpyAsync(e->h_ev_out, &e->d_ctr_ev->evict_out, 8, cudaMemcpyDeviceToHost, e->evict_stream));
     CU(cudaStreamSynchronize(e->evict_stream));
     if (*e->h_ev_out != live)
         return fail(FA_E_CUDA, "fa_evict: table scan found %llu flows, counter says %llu", *e->h_ev_out, (unsigned long long)live);
-    if (k != PTR_DEVICE) {
+    if (!feats && k != PTR_DEVICE) {
         if (o->present) memset(o->present, 0, live);
         if (o->dns) memset(o->dns, 0, live * 64);
         if (o->additional) memset(o->additional, 0, live * 32);
@@ -931,7 +987,7 @@ static int evict_swapped(fa_engine* e, const fa_evict_out* o, size_t cap, size_t
     {
         std::lock_guard<std::mutex> lk(e->mu);
         e->st.kernel_launches += launched;
-        if (k != PTR_DEVICE) e->st.d2h_bytes += live * fa::kRecBytes;
+        e->st.d2h_bytes += d2h;
     }
     *n_out = (size_t)live;
     return FA_OK;
@@ -952,63 +1008,10 @@ int fa_evict_ex(fa_engine* e, const fa_evict_out* o, size_t cap, size_t* n_out) 
     if (!out_records) return fail(FA_E_INVAL, "fa_evict: null out_records");
     if (cap < live) return fail(FA_E_2BIG, "fa_evict: capacity %zu < %llu live flows", cap, (unsigned long long)live);
     const bool feats = e->table.feat_add || e->table.feat_dns || e->table.feat_drop;
-    const PtrKind k = classify(out_records);
-    uint8_t* d_out = nullptr;
-    if (k == PTR_DEVICE) {
-        d_out = static_cast<uint8_t*>(out_records);
-    } else {
-        if (e->evict_cap < live) {
-            cudaFree(e->d_evict); e->d_evict = nullptr; e->evict_cap = 0;
-            uint64_t want = std::max<uint64_t>(live, std::min<uint64_t>(e->cfg.max_entries, live * 2));
-            CU(cudaMalloc(&e->d_evict, want * fa::kRecBytes));
-            e->evict_cap = want;
-        }
-        d_out = e->d_evict;
-    }
-    // feature outputs are staged on the device unless the caller handed device pointers
-    uint8_t *d_dns = nullptr, *d_add = nullptr, *d_drop = nullptr, *d_pres = nullptr;
-    unsigned long long* d_rmin = nullptr;
-    if (feats) {
-        if (e->feat_evict_cap < live) {
-            cudaFree(e->d_evict_dns); cudaFree(e->d_evict_add); cudaFree(e->d_evict_present); cudaFree(e->d_slot_of_out);
-            cudaFree(e->d_evict_drop); cudaFree(e->d_evict_rttmin);
-            e->d_evict_dns = e->d_evict_add = e->d_evict_present = e->d_evict_drop = nullptr; e->d_evict_rttmin = nullptr;
-            e->d_slot_of_out = nullptr; e->feat_evict_cap = 0;
-            uint64_t want = std::max<uint64_t>(live, std::min<uint64_t>(e->cfg.max_entries, live * 2));
-            CU(cudaMalloc(&e->d_evict_dns, want * 64)); CU(cudaMalloc(&e->d_evict_add, want * 32));
-            CU(cudaMalloc(&e->d_evict_drop, want * 32)); CU(cudaMalloc(&e->d_evict_rttmin, want * 8));
-            CU(cudaMalloc(&e->d_evict_present, want)); CU(cudaMalloc(&e->d_slot_of_out, want * 4));
-            e->feat_evict_cap = want;
-        }
-        d_dns = out_dns ? (classify(out_dns) == PTR_DEVICE ? static_cast<uint8_t*>(out_dns) : e->d_evict_dns) : nullptr;
-        d_add = out_additional ? (classify(out_additional) == PTR_DEVICE ? static_cast<uint8_t*>(out_additional) : e->d_evict_add) : nullptr;
-        d_drop = o->pkt_drops ? (classify(o->pkt_drops) == PTR_DEVICE ? static_cast<uint8_t*>(o->pkt_drops) : e->d_evict_drop) : nullptr;
-        d_rmin = o->rtt_min ? (classify(o->rtt_min) == PTR_DEVICE ? reinterpret_cast<unsigned long long*>(o->rtt_min) : e->d_evict_rttmin) : nullptr;
-        d_pres = out_present ? (classify(out_present) == PTR_DEVICE ? out_present : e->d_evict_present) : nullptr;
-    }
+    if (int src = evict_staging(e, live, classify(out_records) != PTR_DEVICE, feats)) return src;
     CU(cudaMemsetAsync(&e->d_ctr->evict_out, 0, sizeof(unsigned long long), e->stream));
-    if (e->cfg.mode == FA_MODE_KERNEL_MAP)
-        e->st.kernel_launches += fa::launch_kmap_evict(e->table, e->km_met, d_out, live, &e->d_ctr->evict_out,
-                                                       feats ? e->d_slot_of_out : nullptr, e->sm_count, e->stream);
-    else
-        e->st.kernel_launches += fa::launch_evict(e->table, reinterpret_cast<uint4*>(d_out), feats ? e->d_slot_of_out : nullptr, live,
-                                                  e->d_ctr, e->sm_count, e->stream);
-    if (feats)
-        e->st.kernel_launches += fa::launch_evict_features(e->table, e->d_slot_of_out, live, d_out, d_dns, d_add, d_drop, d_rmin, d_pres,
-                                                           e->sm_count, e->stream);
-    CU(cudaGetLastError());
+    if (int src = evict_scan(e, e->table, o, live, e->d_ctr, e->stream, &e->st.kernel_launches, &e->st.d2h_bytes)) return src;
     CU(cudaMemsetAsync(&e->d_ctr->live, 0, sizeof(unsigned long long), e->stream));
-    if (k != PTR_DEVICE) {
-        CU(cudaMemcpyAsync(out_records, d_out, live * fa::kRecBytes, cudaMemcpyDeviceToHost, e->stream));
-        e->st.d2h_bytes += live * fa::kRecBytes;
-    }
-    if (feats) {
-        if (out_dns && d_dns == e->d_evict_dns) { CU(cudaMemcpyAsync(out_dns, d_dns, live * 64, cudaMemcpyDeviceToHost, e->stream)); e->st.d2h_bytes += live * 64; }
-        if (out_additional && d_add == e->d_evict_add) { CU(cudaMemcpyAsync(out_additional, d_add, live * 32, cudaMemcpyDeviceToHost, e->stream)); e->st.d2h_bytes += live * 32; }
-        if (o->pkt_drops && d_drop == e->d_evict_drop) { CU(cudaMemcpyAsync(o->pkt_drops, d_drop, live * 32, cudaMemcpyDeviceToHost, e->stream)); e->st.d2h_bytes += live * 32; }
-        if (o->rtt_min && d_rmin == e->d_evict_rttmin) { CU(cudaMemcpyAsync(o->rtt_min, d_rmin, live * 8, cudaMemcpyDeviceToHost, e->stream)); e->st.d2h_bytes += live * 8; }
-        if (out_present && d_pres == e->d_evict_present) { CU(cudaMemcpyAsync(out_present, d_pres, live, cudaMemcpyDeviceToHost, e->stream)); e->st.d2h_bytes += live; }
-    }
     CU(cudaMemcpyAsync(e->h_ctr, e->d_ctr, sizeof(fa::Counters), cudaMemcpyDeviceToHost, e->stream));
     CU(cudaStreamSynchronize(e->stream));
     if (e->h_ctr->evict_out != live)

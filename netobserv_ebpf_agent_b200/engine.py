@@ -150,12 +150,14 @@ class FlowAggEngine:
         check(lib().fa_evict(self._h, _ptr(out), None, None, None, cap, C.byref(got)))
         return out[: got.value]
 
-    def evict_ex(self):
+    def evict_ex(self, cap=None):
         """Lookup-and-delete all flows with every block -> records (n,144), dns (n,64), additional (n,32),
-        pkt_drops (n,32), rtt_min (n,) u64, present (n,)."""
+        pkt_drops (n,32), rtt_min (n,) u64, present (n,).
+        cap: output capacity in flows (default: the live count right now; pass max_entries when another thread keeps
+        ingesting, FA_F_NONBLOCKING_EVICT)."""
         from ._lib import EvictOut
-        n = self.live_flows()
-        cap = max(n, 1)
+        if cap is None:
+            cap = max(self.live_flows(), 1)
         out, dns, add = np.zeros((cap, REC_BYTES), np.uint8), np.zeros((cap, 64), np.uint8), np.zeros((cap, 32), np.uint8)
         drops, rmin, pres = np.zeros((cap, 32), np.uint8), np.zeros(cap, np.uint64), np.zeros(cap, np.uint8)
         o = EvictOut(records=out.ctypes.data, dns=dns.ctypes.data, additional=add.ctypes.data, pkt_drops=drops.ctypes.data,
