@@ -204,12 +204,17 @@ int launch_kmap_evict(const Table& t, uint8_t* met, uint8_t* out, unsigned long 
 
 namespace {
 
+// The live-flow count is exactly `live` and no launch is in flight (counters just read back, or the table emptied).
+void set_live_known(fa_engine* e, uint64_t live) {
+    e->live_known = live;
+    e->unsynced_records = 0;
+    e->ring_head = e->ring_tail;
+}
+
 int sync_counters(fa_engine* e) {
     CU(cudaMemcpyAsync(e->h_ctr, e->d_ctr, sizeof(fa::Counters), cudaMemcpyDeviceToHost, e->stream));
     CU(cudaStreamSynchronize(e->stream));
-    e->live_known = e->h_ctr->live;
-    e->unsynced_records = 0;
-    e->ring_head = e->ring_tail;
+    set_live_known(e, e->h_ctr->live);
     return FA_OK;
 }
 
@@ -260,6 +265,19 @@ int launch_chunk(fa_engine* e, const uint8_t* d_recs, uint32_t n) {
     return note_launch(e, n);
 }
 
+// Pre-pass of a chunk that may fill the table: *cut = the index of the first of the n records whose key is new while
+// live_known (exact) flows fill max_entries, or n.  Waits for the 4-byte read-back.
+int find_cut(fa_engine* e, const uint8_t* d_recs, uint32_t n, uint32_t* cut) {
+    e->st.kernel_launches += fa::launch_full_cut(reinterpret_cast<const uint4*>(d_recs), n, e->table, e->live_known,
+                                                 e->cfg.max_entries, e->d_cut_set, e->cut_set_slots, e->d_cut_bitmap,
+                                                 e->d_cut_out, e->sm_count, e->stream);
+    CU(cudaGetLastError());
+    CU(cudaMemcpyAsync(e->h_cut_out, e->d_cut_out, 4, cudaMemcpyDeviceToHost, e->stream));
+    CU(cudaStreamSynchronize(e->stream));
+    *cut = *e->h_cut_out;
+    return FA_OK;
+}
+
 // ACCOUNTER mode: fold a device-resident chunk honouring max_entries.
 // Returns FA_OK (all folded) or FA_FULL with *consumed < n.
 int ingest_chunk_accounter(fa_engine* e, const uint8_t* d_recs, uint32_t n, uint32_t* consumed) {
@@ -295,13 +313,8 @@ int ingest_chunk_accounter(fa_engine* e, const uint8_t* d_recs, uint32_t n, uint
     // caller goes on with the rest of its chunk.
     const uint64_t room = M > e->live_known ? M - e->live_known : 0;      // exact: the counters were just read
     const uint32_t win = (uint32_t)std::min<uint64_t>(n, std::max<uint64_t>(4096, 4 * room));
-    e->st.kernel_launches += fa::launch_full_cut(reinterpret_cast<const uint4*>(d_recs), win, e->table, e->live_known, M,
-                                                 e->d_cut_set, e->cut_set_slots, e->d_cut_bitmap, e->d_cut_out,
-                                                 e->sm_count, e->stream);
-    CU(cudaGetLastError());
-    CU(cudaMemcpyAsync(e->h_cut_out, e->d_cut_out, 4, cudaMemcpyDeviceToHost, e->stream));
-    CU(cudaStreamSynchronize(e->stream));
-    const uint32_t cut = *e->h_cut_out;
+    uint32_t cut = 0;
+    if (int rc = find_cut(e, d_recs, win, &cut)) return rc;
     if (cut > 0) {
         int rc = launch_chunk(e, d_recs, cut);
         if (rc) return rc;
@@ -326,13 +339,7 @@ int ingest_chunk_kmap(fa_engine* e, const uint8_t* d_recs, uint32_t n, uint32_t*
     }
     uint32_t cut = n;                                  // records [cut, n) find the map full
     if (e->live_known + e->unsynced_records + n > M) {
-        e->st.kernel_launches += fa::launch_full_cut(reinterpret_cast<const uint4*>(d_recs), n, e->table, e->live_known, M,
-                                                     e->d_cut_set, e->cut_set_slots, e->d_cut_bitmap, e->d_cut_out,
-                                                     e->sm_count, e->stream);
-        CU(cudaGetLastError());
-        CU(cudaMemcpyAsync(e->h_cut_out, e->d_cut_out, 4, cudaMemcpyDeviceToHost, e->stream));
-        CU(cudaStreamSynchronize(e->stream));
-        cut = *e->h_cut_out;
+        if (int rc = find_cut(e, d_recs, n, &cut)) return rc;
         if (cut < n) e->st.full_cuts++;
     }
     fa::KmParams P{};
@@ -358,17 +365,19 @@ int ingest_chunk(fa_engine* e, const uint8_t* d_recs, uint32_t n, uint32_t* cons
                                              : ingest_chunk_accounter(e, d_recs, n, consumed);
 }
 
+// Fold n device-resident records in launches of at most max_batch; a launch may fold only a window of its records
+// ("full" cuts).  Returns FA_OK or the first error / FA_FULL, with *consumed the records folded.
 int ingest_device(fa_engine* e, const uint8_t* d_recs, size_t n, size_t* consumed) {
     size_t done = 0;
-    while (done < n) {
+    int rc = FA_OK;
+    while (rc == FA_OK && done < n) {
         const uint32_t c = (uint32_t)std::min<size_t>(n - done, e->max_batch);
         uint32_t took = 0;
-        int rc = ingest_chunk(e, d_recs + done * fa::kRecBytes, c, &took);
+        rc = ingest_chunk(e, d_recs + done * fa::kRecBytes, c, &took);
         done += took;
-        if (rc != FA_OK) { if (consumed) *consumed = done; return rc; }
     }
-    if (consumed) *consumed = done;
-    return FA_OK;
+    *consumed = done;
+    return rc;
 }
 
 // Host data reaches the device through two staging buffers of stage_records() records: the copy of chunk k+1 (copy
@@ -376,71 +385,82 @@ int ingest_device(fa_engine* e, const uint8_t* d_recs, size_t n, size_t* consume
 // launch size for device-resident input: a large launch amortises K1's start-up, a small stage keeps the pipeline fine.
 static uint64_t stage_records(const fa_engine* e) { return std::min<uint64_t>(e->max_batch, 1ull << 20); }   // 151 MB of records per copy
 
-static int stage_alloc(fa_engine* e, bool pageable) {
-    for (int i = 0; i < 2; i++) {
-        if (!e->d_stage[i]) CU(cudaMalloc(&e->d_stage[i], stage_records(e) * fa::kRecBytes));
-        if (pageable && !e->h_stage[i]) CU(cudaHostAlloc(&e->h_stage[i], stage_records(e) * fa::kRecBytes, cudaHostAllocDefault));
-    }
-    return FA_OK;
+// ACCOUNTER mode: a cache that is about to fill cuts the chunk after roughly `room` new keys.  A chunk of c items is
+// bounded by a window proportional to the room left, so that a "full" return does not leave most of a copied or
+// expanded chunk unused (the caller hands the rest in again after its eviction).
+static uint64_t room_window(fa_engine* e, uint64_t c) {
+    if (e->cfg.mode != FA_MODE_ACCOUNTER || (e->cfg.flags & FA_F_NO_FULL_CUT)) return c;
+    retire_completed(e);
+    const uint64_t used = e->live_known + e->unsynced_records;
+    const uint64_t room = e->cfg.max_entries > used ? e->cfg.max_entries - used : 0;
+    return room < c ? std::min<uint64_t>(c, std::max<uint64_t>(4096, 4 * room)) : c;
 }
 
-// Copy `bytes` of host data into the next staging buffer; the engine stream waits for the copy.  -> *sidx for stage_release.
-static int stage_copy(fa_engine* e, const uint8_t* src, size_t bytes, bool pinned, int* sidx_out) {
-    const int sidx = e->stage_cur; e->stage_cur ^= 1;
-    CU(cudaEventSynchronize(e->ev_stage_free[sidx]));                // previous consumer of this stage is done
-    if (!pinned) { memcpy(e->h_stage[sidx], src, bytes); src = e->h_stage[sidx]; }
-    CU(cudaMemcpyAsync(e->d_stage[sidx], src, bytes, cudaMemcpyHostToDevice, e->copy_stream));
-    CU(cudaEventRecord(e->ev_copied[sidx], e->copy_stream));
-    CU(cudaStreamWaitEvent(e->stream, e->ev_copied[sidx], 0));
-    e->st.h2d_bytes += bytes;
-    *sidx_out = sidx;
-    return FA_OK;
-}
+enum RoomWindow { WINDOW_NONE, WINDOW_HOST, WINDOW_ALL };   // which input room_window() bounds
 
-static int stage_release(fa_engine* e, int sidx) {                   // the kernels enqueued so far were the stage's last readers
-    CU(cudaEventRecord(e->ev_stage_free[sidx], e->stream));
-    return FA_OK;
-}
-
-int ingest_host(fa_engine* e, const uint8_t* h_recs, size_t n, size_t* consumed, bool pinned) {
+// The input of an fa_ingest* call: n items of `width` bytes in caller memory, handed to the kernels in chunks of at most
+// dev_chunk items (device input, read in place) or host_chunk items (host input, copied into a staging buffer).  Per
+// chunk: next(), release() right after the last kernel that reads the chunk is enqueued, advance() by the items
+// consumed.  finish() once at the end.
+struct Input {
+    fa_engine* e;
+    const uint8_t* src;
+    size_t n, width;
+    uint64_t dev_chunk, host_chunk;
+    RoomWindow window;
+    PtrKind kind;
     size_t done = 0;
-    int rc = FA_OK;
-    while (done < n) {
-        uint32_t c = (uint32_t)std::min<size_t>(n - done, stage_records(e));
-        if (e->cfg.mode == FA_MODE_ACCOUNTER && !(e->cfg.flags & FA_F_NO_FULL_CUT)) {
-            // A cache that is about to fill cuts the chunk after roughly `room` new keys: stage a window proportional
-            // to the room left, so that a "full" return does not leave most of a copied chunk unused (the caller
-            // hands the rest in again after its eviction).
-            retire_completed(e);
-            const uint64_t used = e->live_known + e->unsynced_records;
-            const uint64_t room = e->cfg.max_entries > used ? e->cfg.max_entries - used : 0;
-            if (room < c) c = (uint32_t)std::min<uint64_t>(c, std::max<uint64_t>(4096, 4 * room));
-        }
-        int sidx = 0;
-        if (int src_rc = stage_copy(e, h_recs + done * fa::kRecBytes, (size_t)c * fa::kRecBytes, pinned, &sidx)) return src_rc;
-        uint32_t off = 0;                                            // a chunk may be folded in several windows
-        while (off < c) {
-            uint32_t took = 0;
-            rc = ingest_chunk(e, e->d_stage[sidx] + (size_t)off * fa::kRecBytes, c - off, &took);
-            off += took;
-            if (rc != FA_OK) break;
-        }
-        if (int rel_rc = stage_release(e, sidx)) return rel_rc;
-        done += off;
-        if (rc != FA_OK) break;
+    int sidx = -1;                                             // staging buffer of the current chunk (host input)
+
+    Input(fa_engine* e_, const void* p, size_t n_, size_t width_, uint64_t dev_chunk_, uint64_t host_chunk_, RoomWindow window_)
+        : e(e_), src(static_cast<const uint8_t*>(p)), n(n_), width(width_), dev_chunk(dev_chunk_), host_chunk(host_chunk_),
+          window(window_), kind(classify(p)) {}
+
+    bool misaligned(uintptr_t align) const { return kind == PTR_DEVICE && (reinterpret_cast<uintptr_t>(src) & (align - 1)); }
+    bool more() const { return done < n; }
+    void advance(size_t k) { done += k; }
+
+    uint64_t chunk() const {                                   // items in the next chunk
+        const uint64_t c = std::min<uint64_t>(n - done, kind == PTR_DEVICE ? dev_chunk : host_chunk);
+        return window == WINDOW_ALL || (window == WINDOW_HOST && kind != PTR_DEVICE) ? room_window(e, c) : c;
     }
-    // the caller's buffer must not be referenced after return
-    CU(cudaStreamSynchronize(e->copy_stream));
-    if (consumed) *consumed = done;
-    return rc;
-}
+
+    // -> the next chunk on the device and its item count.  Host input is copied into the next staging buffer on the
+    // copy stream (pageable input through a pinned buffer first); the engine stream waits for the copy.
+    int next(const uint8_t** d_in, uint64_t* c) {
+        *c = chunk();
+        const uint8_t* p = src + done * width;
+        *d_in = p;
+        if (kind == PTR_DEVICE) return FA_OK;
+        const size_t bytes = *c * width, stage_bytes = stage_records(e) * fa::kRecBytes;
+        for (int i = 0; i < 2; i++) {
+            if (!e->d_stage[i]) CU(cudaMalloc(&e->d_stage[i], stage_bytes));
+            if (kind == PTR_PAGEABLE && !e->h_stage[i]) CU(cudaHostAlloc(&e->h_stage[i], stage_bytes, cudaHostAllocDefault));
+        }
+        sidx = e->stage_cur; e->stage_cur ^= 1;
+        CU(cudaEventSynchronize(e->ev_stage_free[sidx]));            // the previous reader of this stage is done
+        if (kind == PTR_PAGEABLE) { memcpy(e->h_stage[sidx], p, bytes); p = e->h_stage[sidx]; }
+        CU(cudaMemcpyAsync(e->d_stage[sidx], p, bytes, cudaMemcpyHostToDevice, e->copy_stream));
+        CU(cudaEventRecord(e->ev_copied[sidx], e->copy_stream));
+        CU(cudaStreamWaitEvent(e->stream, e->ev_copied[sidx], 0));
+        e->st.h2d_bytes += bytes;
+        *d_in = e->d_stage[sidx];
+        return FA_OK;
+    }
+
+    int release() {                                            // the kernels enqueued so far were the chunk's last readers
+        if (sidx >= 0) CU(cudaEventRecord(e->ev_stage_free[sidx], e->stream));
+        return FA_OK;
+    }
+
+    int finish(int rc, size_t* consumed) {
+        if (kind != PTR_DEVICE) CU(cudaStreamSynchronize(e->copy_stream));   // the caller's buffer is not referenced after return
+        if (consumed) *consumed = done;
+        return rc;
+    }
+};
 
 }  // namespace
-
-static uint64_t e_max_batch_tmp(const fa_config* cfg) {
-    uint64_t mb = cfg->max_batch ? cfg->max_batch : (1ull << 22);
-    return mb > (1ull << 28) ? (1ull << 28) : mb;
-}
 
 // Everything fa_evict swaps (FA_F_NONBLOCKING_EVICT): identity lines, occupancy bitmap, the mode's metric lines (hot
 // lines / KERNEL_MAP flow_metrics lines) and the enabled feature lines — zeroed on the engine stream.
@@ -548,7 +568,7 @@ int fa_create(const fa_config* cfg, fa_engine** out) {
         CU(cudaHostAlloc(&e->h_km_ctr, sizeof(fa::KmCounters), cudaHostAllocDefault));
         memset(e->h_km_ctr, 0, sizeof(fa::KmCounters));
     }
-    if (cfg->flags & feat_flags) CU(cudaMalloc(&e->d_slot_of, e_max_batch_tmp(cfg) * 4));
+    if (cfg->flags & feat_flags) CU(cudaMalloc(&e->d_slot_of, e->max_batch * 4));
     CU(cudaMalloc(&e->d_ctr, sizeof(fa::Counters)));
     CU(cudaMemsetAsync(e->d_ctr, 0, sizeof(fa::Counters), e->stream));
     CU(cudaHostAlloc(&e->h_ctr, sizeof(fa::Counters), cudaHostAllocDefault));
@@ -661,13 +681,20 @@ int fa_ingest(fa_engine* e, const void* recs, size_t n, size_t* consumed) {
     if (!recs) return fail(FA_E_INVAL, "fa_ingest: null records");
     std::lock_guard<std::mutex> lk(e->mu);
     CU(cudaSetDevice(e->device));
-    const PtrKind k = classify(recs);
-    if (k == PTR_DEVICE) {
-        if (reinterpret_cast<uintptr_t>(recs) & 15) return fail(FA_E_INVAL, "fa_ingest: device records must be 16-byte aligned");
-        return ingest_device(e, static_cast<const uint8_t*>(recs), n, consumed);
+    // device records are folded in one go (ingest_device launches by max_batch); host records stage by stage
+    Input in(e, recs, n, fa::kRecBytes, SIZE_MAX, stage_records(e), WINDOW_HOST);
+    if (in.misaligned(16)) return fail(FA_E_INVAL, "fa_ingest: device records must be 16-byte aligned");
+    int rc = FA_OK;
+    while (rc == FA_OK && in.more()) {
+        const uint8_t* d_recs = nullptr;
+        uint64_t c = 0;
+        size_t took = 0;
+        if (int src_rc = in.next(&d_recs, &c)) return src_rc;
+        rc = ingest_device(e, d_recs, c, &took);
+        if (int rel_rc = in.release()) return rel_rc;
+        in.advance(took);
     }
-    if (int rc = stage_alloc(e, k == PTR_PAGEABLE)) return rc;
-    return ingest_host(e, static_cast<const uint8_t*>(recs), n, consumed, k == PTR_PINNED);
+    return in.finish(rc, consumed);
 }
 
 int fa_ingest_events(fa_engine* e, const void* events, size_t n, size_t* consumed) {
@@ -678,45 +705,23 @@ int fa_ingest_events(fa_engine* e, const void* events, size_t n, size_t* consume
     static_assert(sizeof(fa_packet_event) == 64, "fa_packet_event ABI");
     std::lock_guard<std::mutex> lk(e->mu);
     CU(cudaSetDevice(e->device));
-    const PtrKind k = classify(events);
-    if (k == PTR_DEVICE && (reinterpret_cast<uintptr_t>(events) & 15)) return fail(FA_E_INVAL, "fa_ingest_events: device events must be 16-byte aligned");
+    Input in(e, events, n, 64, e->max_batch, stage_records(e), WINDOW_ALL);
+    if (in.misaligned(16)) return fail(FA_E_INVAL, "fa_ingest_events: device events must be 16-byte aligned");
     if (!e->d_expanded) CU(cudaMalloc(&e->d_expanded, e->max_batch * fa::kRecBytes));
-    if (k != PTR_DEVICE) { if (int arc = stage_alloc(e, k == PTR_PAGEABLE)) return arc; }
-    size_t done = 0;
+    // the expansion and K1 of successive chunks are ordered on the engine's stream, so one d_expanded is enough
     int rc = FA_OK;
-    while (done < n) {
-        uint32_t c = (uint32_t)std::min<size_t>(n - done, k == PTR_DEVICE ? e->max_batch : stage_records(e));
-        if (e->cfg.mode == FA_MODE_ACCOUNTER && !(e->cfg.flags & FA_F_NO_FULL_CUT)) {     // see ingest_host: stage by the room left
-            retire_completed(e);
-            const uint64_t used = e->live_known + e->unsynced_records;
-            const uint64_t room = e->cfg.max_entries > used ? e->cfg.max_entries - used : 0;
-            if (room < c) c = (uint32_t)std::min<uint64_t>(c, std::max<uint64_t>(4096, 4 * room));
-        }
-        const uint8_t* src = static_cast<const uint8_t*>(events) + done * 64;
-        const uint8_t* d_ev = src;
-        // host events: staged like fa_ingest's records (the copy of the next chunk overlaps this chunk's kernels); the
-        // expansion and K1 of successive chunks are ordered on the engine's stream, so one d_expanded is enough
-        int sidx = -1;
-        if (k != PTR_DEVICE) {
-            if (int src_rc = stage_copy(e, src, (size_t)c * 64, k == PTR_PINNED, &sidx)) return src_rc;
-            d_ev = e->d_stage[sidx];
-        }
+    while (rc == FA_OK && in.more()) {
+        const uint8_t* d_ev = nullptr;
+        uint64_t c = 0;
+        size_t took = 0;
+        if (int src_rc = in.next(&d_ev, &c)) return src_rc;
         e->st.kernel_launches += fa::launch_expand_events(reinterpret_cast<const uint4*>(d_ev), c, reinterpret_cast<uint4*>(e->d_expanded), e->stream);
         CU(cudaGetLastError());
-        if (sidx >= 0) { if (int rel_rc = stage_release(e, sidx)) return rel_rc; }
-        uint32_t off = 0;
-        while (off < c) {                                   // a chunk may be folded in several windows ("full" cuts)
-            uint32_t took = 0;
-            rc = ingest_chunk(e, e->d_expanded + (size_t)off * fa::kRecBytes, c - off, &took);
-            off += took;
-            if (rc != FA_OK) break;
-        }
-        done += off;
-        if (rc != FA_OK) break;
+        if (int rel_rc = in.release()) return rel_rc;
+        rc = ingest_device(e, e->d_expanded, c, &took);
+        in.advance(took);
     }
-    if (k != PTR_DEVICE) CU(cudaStreamSynchronize(e->copy_stream));   // the caller's buffer must not be referenced after return
-    if (consumed) *consumed = done;
-    return rc;
+    return in.finish(rc, consumed);
 }
 
 int fa_ingest_snaps(fa_engine* e, const void* snaps, size_t n, uint32_t stride, size_t* consumed) {
@@ -727,33 +732,25 @@ int fa_ingest_snaps(fa_engine* e, const void* snaps, size_t n, uint32_t stride, 
     if (!snaps) return fail(FA_E_INVAL, "fa_ingest_snaps: null snapshots");
     std::lock_guard<std::mutex> lk(e->mu);
     CU(cudaSetDevice(e->device));
-    const PtrKind k = classify(snaps);
-    if (k == PTR_DEVICE && (reinterpret_cast<uintptr_t>(snaps) & 7)) return fail(FA_E_INVAL, "fa_ingest_snaps: device snapshots must be 8-byte aligned");
+    // host chunks are bounded by the staging buffers (stage_records() x 144 bytes), device chunks by max_batch records
+    Input in(e, snaps, n, stride, e->max_batch, std::min<uint64_t>(e->max_batch, stage_records(e) * fa::kRecBytes / stride), WINDOW_NONE);
+    if (in.misaligned(8)) return fail(FA_E_INVAL, "fa_ingest_snaps: device snapshots must be 8-byte aligned");
     if (!e->d_expanded) CU(cudaMalloc(&e->d_expanded, e->max_batch * fa::kRecBytes));
     if (!e->d_snap_src) CU(cudaMalloc(&e->d_snap_src, e->max_batch * sizeof(uint32_t)));
     if (!e->d_snap_cnt) CU(cudaMalloc(&e->d_snap_cnt, (fa::kSnapMaxCtas + 8) * sizeof(uint32_t)));
     if (e->filter.n_rules && !e->d_snap_verdict) CU(cudaMalloc(&e->d_snap_verdict, e->max_batch));
-    if (k != PTR_DEVICE) { if (int arc = stage_alloc(e, k == PTR_PAGEABLE)) return arc; }
     unsigned long long* d_total = reinterpret_cast<unsigned long long*>(e->d_snap_cnt + fa::kSnapMaxCtas);
-    // host chunks are bounded by the staging buffers (stage_records() x 144 bytes), device chunks by max_batch records
-    const size_t per_chunk = k == PTR_DEVICE ? e->max_batch : std::min<uint64_t>(e->max_batch, stage_records(e) * fa::kRecBytes / stride);
-    size_t done = 0;
     int rc = FA_OK;
-    while (done < n) {
-        const uint32_t c = (uint32_t)std::min<size_t>(n - done, per_chunk);
-        const uint8_t* src = static_cast<const uint8_t*>(snaps) + done * stride;
-        const uint8_t* d_sn = src;
-        int sidx = -1;
-        if (k != PTR_DEVICE) {
-            if (int src_rc = stage_copy(e, src, (size_t)c * stride, k == PTR_PINNED, &sidx)) return src_rc;
-            d_sn = e->d_stage[sidx];
-        }
+    while (in.more()) {
+        const uint8_t* d_sn = nullptr;
+        uint64_t c = 0;
+        if (int src_rc = in.next(&d_sn, &c)) return src_rc;
         CU(cudaMemsetAsync(d_total + 1, 0, 24, e->stream));             // the filter's three counters of this chunk
         e->st.kernel_launches += fa::launch_parse_snaps(d_sn, c, stride, &e->filter, e->d_snap_cnt, e->d_snap_verdict,
                                                         reinterpret_cast<uint4*>(e->d_expanded), e->d_snap_src, d_total, d_total + 1,
                                                         e->sm_count, e->stream);
         CU(cudaGetLastError());
-        if (sidx >= 0) { if (int rel_rc = stage_release(e, sidx)) return rel_rc; }
+        if (int rel_rc = in.release()) return rel_rc;
         // how many packets were submitted decides the launch sizes of the fold: one 8-byte read-back per chunk
         unsigned long long back[4] = {0, 0, 0, 0};                      // submitted + kept | filter accept / reject / no match
         CU(cudaMemcpyAsync(back, d_total, 32, cudaMemcpyDeviceToHost, e->stream));
@@ -762,13 +759,8 @@ int fa_ingest_snaps(fa_engine* e, const void* snaps, size_t n, uint32_t stride, 
         e->st.filter_accept += back[1]; e->st.filter_reject += back[2]; e->st.filter_nomatch += back[3];
         // every submitted packet bumps exactly one of the three counters: what the filter skipped = submitted - kept
         const uint64_t filtered_out = e->filter.n_rules ? back[1] + back[2] + back[3] - (uint64_t)m : 0;
-        uint32_t off = 0;
-        while (off < m) {                                   // a chunk may be folded in several windows ("full" cuts)
-            uint32_t took = 0;
-            rc = ingest_chunk(e, e->d_expanded + (size_t)off * fa::kRecBytes, m - off, &took);
-            off += took;
-            if (rc != FA_OK) break;
-        }
+        size_t off = 0;
+        rc = ingest_device(e, e->d_expanded, m, &off);
         if (rc == FA_FULL && off < m) {
             // the cut is reported in snapshots: everything before the first record that was not folded, discarded ones included
             uint32_t first_left = 0;
@@ -778,17 +770,15 @@ int fa_ingest_snaps(fa_engine* e, const void* snaps, size_t n, uint32_t stride, 
             // (with a filter the discarded / filtered split of a partially consumed chunk is not known: both count as discarded)
             e->st.snaps_ingested += first_left;
             e->st.snaps_discarded += first_left - off;
-            done += first_left;
+            in.advance(first_left);
             break;
         }
         if (rc != FA_OK) break;
         e->st.snaps_ingested += c;
         e->st.snaps_discarded += c - m - filtered_out;                  // fill_ethhdr's DISCARDs; the filter's skips are in its counters
-        done += c;
+        in.advance(c);
     }
-    if (k != PTR_DEVICE) CU(cudaStreamSynchronize(e->copy_stream));   // the caller's buffer must not be referenced after return
-    if (consumed) *consumed = done;
-    return rc;
+    return in.finish(rc, consumed);
 }
 
 int fa_set_flow_filter(fa_engine* e, const fa_filter_rule* rules, size_t n_rules, const fa_filter_cidr* peers, size_t n_peers) {
@@ -822,6 +812,27 @@ int fa_set_flow_filter(fa_engine* e, const fa_filter_rule* rules, size_t n_rules
     return FA_OK;
 }
 
+// Feature samples may create flows: refuse n more (`what`: samples or packets) when they could take the table past 7/8
+// of its slots.
+static int check_sample_room(fa_engine* e, size_t n, const char* who, const char* what) {
+    if (int rc = sync_counters(e)) return rc;
+    if (e->live_known + n > e->slots - e->slots / 8)
+        return fail(FA_E_2BIG, "%s: %zu %s could overfill the flow table (%llu live of %llu slots): evict first", who, n, what,
+                    (unsigned long long)e->live_known, (unsigned long long)e->slots);
+    return FA_OK;
+}
+
+// Fold m device-resident feature samples of `kind` (0 additional, 1 DNS, 2 packet drops) into the table.
+static int fold_samples(fa_engine* e, int kind, const uint8_t* d_samples, uint32_t m) {
+    e->st.kernel_launches += fa::launch_feature_fold(kind, d_samples, m, e->table, ++e->epoch, e->feat_seq[kind], e->d_slot_of,
+                                                     e->d_ctr, e->sm_count, e->stream);
+    CU(cudaGetLastError());
+    e->feat_seq[kind] += m;
+    e->unsynced_records += m;
+    (kind == 0 ? e->st.additional_ingested : kind == 1 ? e->st.dns_ingested : e->st.pkt_drops_ingested) += m;
+    return FA_OK;
+}
+
 static int ingest_feature(fa_engine* e, int kind, const void* recs, size_t n, const char* who) {
     const uint32_t flag = kind == 0 ? FA_F_ENABLE_RTT : kind == 1 ? FA_F_ENABLE_DNS : FA_F_ENABLE_PKT_DROP;
     if (!e) return fail(FA_E_INVAL, "%s: null engine", who);
@@ -831,36 +842,18 @@ static int ingest_feature(fa_engine* e, int kind, const void* recs, size_t n, co
     std::lock_guard<std::mutex> lk(e->mu);
     CU(cudaSetDevice(e->device));
     const size_t rec_bytes = kind == 1 ? fa::kDnsRecBytes : fa::kAddRecBytes;      // additional and packet-drop samples: 72 B
-    const PtrKind k = classify(recs);
-    if (k == PTR_DEVICE && (reinterpret_cast<uintptr_t>(recs) & 7)) return fail(FA_E_INVAL, "%s: device records must be 8-byte aligned", who);
-    // feature samples may create flows: never let the table pass 7/8 of its slots
-    int rc = sync_counters(e);
-    if (rc) return rc;
-    if (e->live_known + n > e->slots - e->slots / 8)
-        return fail(FA_E_2BIG, "%s: %zu samples could overfill the flow table (%llu live of %llu slots): evict first", who, n,
-                    (unsigned long long)e->live_known, (unsigned long long)e->slots);
-    if (k != PTR_DEVICE) { if (int arc = stage_alloc(e, k == PTR_PAGEABLE)) return arc; }
-    size_t done = 0;
-    while (done < n) {
-        const uint32_t c = (uint32_t)std::min<size_t>(n - done, k == PTR_DEVICE ? e->max_batch : stage_records(e));
-        const uint8_t* src = static_cast<const uint8_t*>(recs) + done * rec_bytes;
-        const uint8_t* d = src;
-        int sidx = -1;
-        if (k != PTR_DEVICE) {
-            if (int src_rc = stage_copy(e, src, (size_t)c * rec_bytes, k == PTR_PINNED, &sidx)) return src_rc;
-            d = e->d_stage[sidx];
-        }
-        e->st.kernel_launches += fa::launch_feature_fold(kind, d, c, e->table, ++e->epoch, e->feat_seq[kind], e->d_slot_of,
-                                                         e->d_ctr, e->sm_count, e->stream);
-        CU(cudaGetLastError());
-        e->feat_seq[kind] += c;
-        e->unsynced_records += c;
-        if (kind == 0) e->st.additional_ingested += c; else if (kind == 1) e->st.dns_ingested += c; else e->st.pkt_drops_ingested += c;
-        if (sidx >= 0) { if (int rel_rc = stage_release(e, sidx)) return rel_rc; }
-        done += c;
+    Input in(e, recs, n, rec_bytes, e->max_batch, stage_records(e), WINDOW_NONE);
+    if (in.misaligned(8)) return fail(FA_E_INVAL, "%s: device records must be 8-byte aligned", who);
+    if (int rc = check_sample_room(e, n, who, "samples")) return rc;
+    while (in.more()) {
+        const uint8_t* d = nullptr;
+        uint64_t c = 0;
+        if (int rc = in.next(&d, &c)) return rc;
+        if (int rc = fold_samples(e, kind, d, c)) return rc;
+        if (int rc = in.release()) return rc;
+        in.advance(c);
     }
-    if (k != PTR_DEVICE) CU(cudaStreamSynchronize(e->copy_stream));   // the caller's buffer is not referenced after return
-    return FA_OK;
+    return in.finish(FA_OK, nullptr);
 }
 
 int fa_ingest_additional(fa_engine* e, const void* recs, size_t n) { return ingest_feature(e, 0, recs, n, "fa_ingest_additional"); }
@@ -878,7 +871,7 @@ int fa_live_flows(fa_engine* e, size_t* n) {
 }
 
 // Device staging of the host-bound blocks of fa_evict_ex and the slot list of the feature pass, grown on demand.  Only
-// eviction touches it (the blocking path under `mu`, evict_swapped under `evict_mu` alone), never fa_ingest*.
+// eviction touches it (the blocking path under `mu`, the non-blocking one under `evict_mu` alone), never fa_ingest*.
 static int evict_staging(fa_engine* e, uint64_t live, bool records, bool feats) {
     const uint64_t want = std::max<uint64_t>(live, std::min<uint64_t>(e->cfg.max_entries, live * 2));
     if (records && e->evict_cap < live) {
@@ -901,8 +894,9 @@ static int evict_staging(fa_engine* e, uint64_t live, bool records, bool feats) 
 
 // Lookup-and-delete the `live` flows of `t` into the blocks of `o`, on stream `st`: the table scan (K2, or the
 // KERNEL_MAP scan) with ctr->evict_out as its cursor, the feature pass when `t` has feature lines, then the copies of
-// the blocks that are host memory (device blocks are written in place; staging from evict_staging).  The feature
-// blocks of a table without feature lines are not written.  Adds the kernels launched and the bytes copied.
+// the blocks that are host memory (device blocks are written in place; staging from evict_staging).  Every requested
+// block the table does not produce comes out zero, whichever memory it is in.  Adds the kernels launched and the bytes
+// copied.
 static int evict_scan(fa_engine* e, const fa::Table& t, const fa_evict_out* o, uint64_t live, fa::Counters* ctr,
                       cudaStream_t st, uint64_t* launches, uint64_t* d2h) {
     const bool feats = t.feat_add || t.feat_dns || t.feat_drop;
@@ -914,10 +908,20 @@ static int evict_scan(fa_engine* e, const fa::Table& t, const fa_evict_out* o, u
     if (feats) {
         d_dns = dev(o->dns, e->d_evict_dns); d_add = dev(o->additional, e->d_evict_add); d_drop = dev(o->pkt_drops, e->d_evict_drop);
         d_rmin = dev(o->rtt_min, e->d_evict_rttmin); d_pres = dev(o->present, e->d_evict_present);
-        // the block of a feature this engine does not fold comes out zero (the feature pass does not write it)
+        // the block of a feature this engine does not fold is zeroed where the kernels write (the feature pass does not
+        // write it) and copied like the others
         if (d_dns && !t.feat_dns) CU(cudaMemsetAsync(d_dns, 0, live * 64, st));
         if (d_add && !t.feat_add) CU(cudaMemsetAsync(d_add, 0, live * 32, st));
         if (d_drop && !t.feat_drop) CU(cudaMemsetAsync(d_drop, 0, live * 32, st));
+    } else {
+        // no feature pass: every feature block is zeroed where it is
+        const struct { void* p; size_t width; } unmade[5] = {
+            {o->dns, 64}, {o->additional, 32}, {o->pkt_drops, 32}, {o->rtt_min, 8}, {o->present, 1}};
+        for (const auto& b : unmade) {
+            if (!b.p) continue;
+            if (classify(b.p) == PTR_DEVICE) CU(cudaMemsetAsync(b.p, 0, live * b.width, st));
+            else memset(b.p, 0, live * b.width);
+        }
     }
     uint32_t* slot_of_out = feats ? e->d_slot_of_out : nullptr;
     if (e->cfg.mode == FA_MODE_KERNEL_MAP)
@@ -939,92 +943,63 @@ static int evict_scan(fa_engine* e, const fa::Table& t, const fa_evict_out* o, u
     return FA_OK;
 }
 
-// FA_F_NONBLOCKING_EVICT: swap the tables under `mu` (fa_ingest* goes on at once, into the empty one), then lookup-and-
-// delete the retired table on the eviction stream: the scan, the feature pass and the copies to the host.  Only the
-// launches already queued are waited for.  Not swapped: the DNS correlation table, the fallback ring, the KERNEL_MAP
-// counters.
-static int evict_swapped(fa_engine* e, const fa_evict_out* o, size_t cap, size_t* n_out) {
-    std::lock_guard<std::mutex> elk(e->evict_mu);
-    CU(cudaSetDevice(e->device));
-    fa::Table retired{};
-    uint64_t live = 0;
-    {
-        std::lock_guard<std::mutex> lk(e->mu);
-        int rc = sync_counters(e);                     // the queued folds finish; exact live count
-        if (rc) return rc;
-        live = e->live_known;
-        e->st.evictions++;
-        if (live == 0) return FA_OK;
-        if (!o->records) return fail(FA_E_INVAL, "fa_evict: null out_records");
-        if (cap < live) return fail(FA_E_2BIG, "fa_evict: capacity %zu < %llu live flows", cap, (unsigned long long)live);
-        retired = e->table;
-        e->table = e->table_spare;                     // empty: the previous eviction deleted every flow in place
-        e->table_spare = retired;
-        CU(cudaMemsetAsync(&e->d_ctr->live, 0, sizeof(unsigned long long), e->stream));
-        CU(cudaEventRecord(e->ev_swap, e->stream));
-        e->live_known = 0; e->unsynced_records = 0; e->ring_head = e->ring_tail;
-        e->st.flows_evicted += live;
-    }
-    // from here on fa_ingest* runs concurrently, into the new table; this side has its own stream, cursor and staging
-    const bool feats = retired.feat_add || retired.feat_dns || retired.feat_drop;
-    const PtrKind k = classify(o->records);
-    if (int rc = evict_staging(e, live, k != PTR_DEVICE, feats)) return rc;
-    CU(cudaStreamWaitEvent(e->evict_stream, e->ev_swap, 0));
-    CU(cudaMemsetAsync(&e->d_ctr_ev->evict_out, 0, sizeof(unsigned long long), e->evict_stream));
-    uint64_t launched = 0, d2h = 0;
-    if (int rc = evict_scan(e, retired, o, live, e->d_ctr_ev, e->evict_stream, &launched, &d2h)) return rc;
-    CU(cudaMemcpyAsync(e->h_ev_out, &e->d_ctr_ev->evict_out, 8, cudaMemcpyDeviceToHost, e->evict_stream));
-    CU(cudaStreamSynchronize(e->evict_stream));
-    if (*e->h_ev_out != live)
-        return fail(FA_E_CUDA, "fa_evict: table scan found %llu flows, counter says %llu", *e->h_ev_out, (unsigned long long)live);
-    if (!feats && k != PTR_DEVICE) {
-        if (o->present) memset(o->present, 0, live);
-        if (o->dns) memset(o->dns, 0, live * 64);
-        if (o->additional) memset(o->additional, 0, live * 32);
-        if (o->pkt_drops) memset(o->pkt_drops, 0, live * 32);
-        if (o->rtt_min) memset(o->rtt_min, 0, live * 8);
-    }
-    {
-        std::lock_guard<std::mutex> lk(e->mu);
-        e->st.kernel_launches += launched;
-        e->st.d2h_bytes += d2h;
-    }
-    *n_out = (size_t)live;
-    return FA_OK;
-}
-
+// Lookup-and-delete every flow.  Blocking: the live table is scanned on the engine stream under `mu`.
+// FA_F_NONBLOCKING_EVICT: the tables are swapped under `mu` (fa_ingest* goes on at once, into the empty one), then the
+// retired table is scanned on the eviction stream, with its own cursor and staging, under `evict_mu` alone; only the
+// launches queued before the swap are waited for.  Not swapped: the DNS correlation table, the fallback ring, the
+// KERNEL_MAP counters.
 int fa_evict_ex(fa_engine* e, const fa_evict_out* o, size_t cap, size_t* n_out) {
     if (n_out) *n_out = 0;
     if (!e || !n_out || !o) return fail(FA_E_INVAL, "fa_evict: null argument");
-    if (e->double_buffered) return evict_swapped(e, o, cap, n_out);
-    void* out_records = o->records; void* out_dns = o->dns; void* out_additional = o->additional; uint8_t* out_present = o->present;
-    std::lock_guard<std::mutex> lk(e->mu);
+    const bool swap = e->double_buffered;
+    std::unique_lock<std::mutex> elk(e->evict_mu, std::defer_lock);   // one eviction at a time
+    if (swap) elk.lock();
+    std::unique_lock<std::mutex> lk(e->mu);
     CU(cudaSetDevice(e->device));
-    int rc = sync_counters(e);
-    if (rc) return rc;
+    if (int rc = sync_counters(e)) return rc;          // the queued folds finish; exact live count
     const uint64_t live = e->live_known;
     e->st.evictions++;
     if (live == 0) return FA_OK;
-    if (!out_records) return fail(FA_E_INVAL, "fa_evict: null out_records");
+    if (!o->records) return fail(FA_E_INVAL, "fa_evict: null out_records");
     if (cap < live) return fail(FA_E_2BIG, "fa_evict: capacity %zu < %llu live flows", cap, (unsigned long long)live);
-    const bool feats = e->table.feat_add || e->table.feat_dns || e->table.feat_drop;
-    if (int src = evict_staging(e, live, classify(out_records) != PTR_DEVICE, feats)) return src;
-    CU(cudaMemsetAsync(&e->d_ctr->evict_out, 0, sizeof(unsigned long long), e->stream));
-    if (int src = evict_scan(e, e->table, o, live, e->d_ctr, e->stream, &e->st.kernel_launches, &e->st.d2h_bytes)) return src;
-    CU(cudaMemsetAsync(&e->d_ctr->live, 0, sizeof(unsigned long long), e->stream));
-    CU(cudaMemcpyAsync(e->h_ctr, e->d_ctr, sizeof(fa::Counters), cudaMemcpyDeviceToHost, e->stream));
-    CU(cudaStreamSynchronize(e->stream));
-    if (e->h_ctr->evict_out != live)
-        return fail(FA_E_CUDA, "fa_evict: table scan found %llu flows, counter says %llu", (unsigned long long)e->h_ctr->evict_out, (unsigned long long)live);
-    if (!feats) {
-        if (out_present && classify(out_present) != PTR_DEVICE) memset(out_present, 0, live);
-        if (out_dns && classify(out_dns) != PTR_DEVICE) memset(out_dns, 0, live * 64);
-        if (out_additional && classify(out_additional) != PTR_DEVICE) memset(out_additional, 0, live * 32);
-        if (o->pkt_drops && classify(o->pkt_drops) != PTR_DEVICE) memset(o->pkt_drops, 0, live * 32);
-        if (o->rtt_min && classify(o->rtt_min) != PTR_DEVICE) memset(o->rtt_min, 0, live * 8);
+    const fa::Table t = e->table;
+    fa::Counters* ctr = e->d_ctr;
+    cudaStream_t st = e->stream;
+    if (swap) {
+        std::swap(e->table, e->table_spare);           // the spare is empty: the previous eviction deleted every flow in place
+        CU(cudaMemsetAsync(&e->d_ctr->live, 0, sizeof(unsigned long long), e->stream));
+        CU(cudaEventRecord(e->ev_swap, e->stream));
+        set_live_known(e, 0);
+        e->st.flows_evicted += live;
+        lk.unlock();                                   // from here on fa_ingest* runs concurrently, into the new table
+        ctr = e->d_ctr_ev;
+        st = e->evict_stream;
     }
-    e->live_known = 0; e->unsynced_records = 0; e->ring_head = e->ring_tail;
-    e->st.flows_evicted += live;
+    const bool feats = t.feat_add || t.feat_dns || t.feat_drop;
+    if (int rc = evict_staging(e, live, classify(o->records) != PTR_DEVICE, feats)) return rc;
+    if (swap) CU(cudaStreamWaitEvent(st, e->ev_swap, 0));
+    CU(cudaMemsetAsync(&ctr->evict_out, 0, sizeof(unsigned long long), st));
+    uint64_t launched = 0, d2h = 0;
+    if (int rc = evict_scan(e, t, o, live, ctr, st, &launched, &d2h)) return rc;
+    const unsigned long long* found = e->h_ev_out;
+    if (swap) {
+        CU(cudaMemcpyAsync(e->h_ev_out, &ctr->evict_out, 8, cudaMemcpyDeviceToHost, st));
+    } else {
+        CU(cudaMemsetAsync(&e->d_ctr->live, 0, sizeof(unsigned long long), st));
+        CU(cudaMemcpyAsync(e->h_ctr, e->d_ctr, sizeof(fa::Counters), cudaMemcpyDeviceToHost, st));
+        found = &e->h_ctr->evict_out;
+    }
+    CU(cudaStreamSynchronize(st));
+    if (*found != live)
+        return fail(FA_E_CUDA, "fa_evict: table scan found %llu flows, counter says %llu", *found, (unsigned long long)live);
+    if (swap) {
+        lk.lock();
+    } else {
+        set_live_known(e, 0);
+        e->st.flows_evicted += live;
+    }
+    e->st.kernel_launches += launched;
+    e->st.d2h_bytes += d2h;
     *n_out = (size_t)live;
     return FA_OK;
 }
@@ -1036,39 +1011,39 @@ int fa_evict(fa_engine* e, void* out_records, void* out_dns, void* out_additiona
     return fa_evict_ex(e, &o, cap, n_out);
 }
 
-int fa_drain_active(fa_engine* e, void* out_records_dev, size_t cap, size_t* n_out) {
-    if (n_out) *n_out = 0;
-    if (!e || !n_out || !out_records_dev) return fail(FA_E_INVAL, "fa_drain_active: null argument");
-    if (classify(out_records_dev) != PTR_DEVICE) return fail(FA_E_INVAL, "fa_drain_active: out_records must be device memory");
-    if (e->table.feat_add || e->table.feat_dns || e->table.feat_drop) return fail(FA_E_INVAL, "fa_drain_active: not available with feature folds enabled");
-    if (e->cfg.mode != FA_MODE_ACCOUNTER) return fail(FA_E_INVAL, "fa_drain_active: ACCOUNTER mode only");
+// Emit and reset the flows touched since the last drain into out_records_dev.  The count goes to *n_dev_out (device
+// memory, nothing waited for) when it is given, else to *n_out after a wait.
+static int drain_active(fa_engine* e, void* out_records_dev, size_t cap, const char* who, size_t* n_out, uint64_t* n_dev_out) {
+    if (e->table.feat_add || e->table.feat_dns || e->table.feat_drop) return fail(FA_E_INVAL, "%s: not available with feature folds enabled", who);
+    if (e->cfg.mode != FA_MODE_ACCOUNTER) return fail(FA_E_INVAL, "%s: ACCOUNTER mode only", who);
     std::lock_guard<std::mutex> lk(e->mu);
     CU(cudaSetDevice(e->device));
     CU(cudaMemsetAsync(&e->d_ctr->evict_out, 0, sizeof(unsigned long long), e->stream));
     e->st.kernel_launches += fa::launch_evict(e->table, static_cast<uint4*>(out_records_dev), nullptr, cap, e->d_ctr,
                                               e->sm_count, e->stream, /*drain=*/true);
     CU(cudaGetLastError());
-    int rc = sync_counters(e);
-    if (rc) return rc;
+    if (n_dev_out) {
+        CU(cudaMemcpyAsync(n_dev_out, &e->d_ctr->evict_out, 8, cudaMemcpyDeviceToDevice, e->stream));
+        return FA_OK;
+    }
+    if (int rc = sync_counters(e)) return rc;
     if (e->h_ctr->evict_out > cap)
-        return fail(FA_E_2BIG, "fa_drain_active: %llu active flows > capacity %zu (flows beyond it were reset but not written)",
+        return fail(FA_E_2BIG, "%s: %llu active flows > capacity %zu (flows beyond it were reset but not written)", who,
                     (unsigned long long)e->h_ctr->evict_out, cap);
     *n_out = (size_t)e->h_ctr->evict_out;
     return FA_OK;
 }
 
+int fa_drain_active(fa_engine* e, void* out_records_dev, size_t cap, size_t* n_out) {
+    if (n_out) *n_out = 0;
+    if (!e || !n_out || !out_records_dev) return fail(FA_E_INVAL, "fa_drain_active: null argument");
+    if (classify(out_records_dev) != PTR_DEVICE) return fail(FA_E_INVAL, "fa_drain_active: out_records must be device memory");
+    return drain_active(e, out_records_dev, cap, "fa_drain_active", n_out, nullptr);
+}
+
 int fa_drain_active_counted(fa_engine* e, void* out_records_dev, size_t cap, uint64_t* n_dev_out) {
     if (!e || !out_records_dev || !n_dev_out) return fail(FA_E_INVAL, "fa_drain_active_counted: null argument");
-    if (e->table.feat_add || e->table.feat_dns || e->table.feat_drop) return fail(FA_E_INVAL, "fa_drain_active_counted: not available with feature folds enabled");
-    if (e->cfg.mode != FA_MODE_ACCOUNTER) return fail(FA_E_INVAL, "fa_drain_active_counted: ACCOUNTER mode only");
-    std::lock_guard<std::mutex> lk(e->mu);
-    CU(cudaSetDevice(e->device));
-    CU(cudaMemsetAsync(&e->d_ctr->evict_out, 0, sizeof(unsigned long long), e->stream));
-    e->st.kernel_launches += fa::launch_evict(e->table, static_cast<uint4*>(out_records_dev), nullptr, cap, e->d_ctr,
-                                              e->sm_count, e->stream, /*drain=*/true);
-    CU(cudaGetLastError());
-    CU(cudaMemcpyAsync(n_dev_out, &e->d_ctr->evict_out, 8, cudaMemcpyDeviceToDevice, e->stream));
-    return FA_OK;
+    return drain_active(e, out_records_dev, cap, "fa_drain_active_counted", nullptr, n_dev_out);
 }
 
 int fa_route_peer(fa_engine* e, const void* recs, const uint64_t* n_dev, size_t max_n, uint32_t n_shards, uint32_t self_shard,
@@ -1189,48 +1164,29 @@ int fa_ingest_dns_packets(fa_engine* e, const void* pkts, size_t n) {
     std::lock_guard<std::mutex> lk(e->mu);
     CU(cudaSetDevice(e->device));
     if (int rc = dnsc_init(e)) return rc;
-    const PtrKind k = classify(pkts);
-    if (k == PTR_DEVICE && (reinterpret_cast<uintptr_t>(pkts) & 7)) return fail(FA_E_INVAL, "%s: device packets must be 8-byte aligned", who);
-    int rc = sync_counters(e);
-    if (rc) return rc;
-    if (e->live_known + n > e->slots - e->slots / 8)          // every packet may add a sample for a new flow
-        return fail(FA_E_2BIG, "%s: %zu packets could overfill the flow table (%llu live of %llu slots): evict first", who, n,
-                    (unsigned long long)e->live_known, (unsigned long long)e->slots);
-    if (k != PTR_DEVICE) { if (int arc = stage_alloc(e, k == PTR_PAGEABLE)) return arc; }
-    size_t done = 0;
-    while (done < n) {
-        // a chunk never takes more than a quarter of the table: with at most max_entries = slots / 4 present keys after a
-        // rebuild the table stays at most half full, so a probe sequence cannot run out
-        const uint64_t cmax = std::min<uint64_t>(e->dnsc_chunk, e->dnsc_slots / 4);
-        const uint32_t c = (uint32_t)std::min<size_t>(n - done, k == PTR_DEVICE ? cmax : std::min<uint64_t>(cmax, stage_records(e)));
-        if (e->dnsc_used + c > e->dnsc_slots / 2) { if (int rrc = dnsc_rebuild(e)) return rrc; }
-        const uint8_t* src = static_cast<const uint8_t*>(pkts) + done * fa::kDnsRecBytes;
-        const uint8_t* d = src;
-        int sidx = -1;
-        if (k != PTR_DEVICE) {
-            if (int src_rc = stage_copy(e, src, (size_t)c * fa::kDnsRecBytes, k == PTR_PINNED, &sidx)) return src_rc;
-            d = e->d_stage[sidx];
-        }
+    // a chunk never takes more than a quarter of the table: with at most max_entries = slots / 4 present keys after a
+    // rebuild the table stays at most half full, so a probe sequence cannot run out
+    const uint64_t cmax = std::min<uint64_t>(e->dnsc_chunk, e->dnsc_slots / 4);
+    Input in(e, pkts, n, fa::kDnsRecBytes, cmax, std::min<uint64_t>(cmax, stage_records(e)), WINDOW_NONE);
+    if (in.misaligned(8)) return fail(FA_E_INVAL, "%s: device packets must be 8-byte aligned", who);
+    if (int rc = check_sample_room(e, n, who, "packets")) return rc;     // every packet may add a sample for a new flow
+    while (in.more()) {
+        if (e->dnsc_used + in.chunk() > e->dnsc_slots / 2) { if (int rc = dnsc_rebuild(e)) return rc; }
+        const uint8_t* d = nullptr;
+        uint64_t c = 0;
+        if (int rc = in.next(&d, &c)) return rc;
         e->st.kernel_launches += fa::launch_dns_correlate(d, c, e->dnsc, e->d_dnsc_state, e->d_dnsc_samples, e->d_dnsc_warps, e->d_dnsc_out,
                                                           e->sm_count, e->stream);
         CU(cudaGetLastError());
-        if (sidx >= 0) { if (int rel_rc = stage_release(e, sidx)) return rel_rc; }
-        if (int src2 = dnsc_sync(e)) return src2;             // how many samples the chunk produced (sizes the fold)
+        if (int rc = in.release()) return rc;
+        if (int rc = dnsc_sync(e)) return rc;                 // how many samples the chunk produced (sizes the fold)
         e->dnsc_used += c;
         const uint32_t m = (uint32_t)e->h_dnsc_ctr[fa::DNSC_EMITTED];
-        if (m) {
-            e->st.kernel_launches += fa::launch_feature_fold(1, e->d_dnsc_out, m, e->table, ++e->epoch, e->feat_seq[1], e->d_slot_of,
-                                                             e->d_ctr, e->sm_count, e->stream);
-            CU(cudaGetLastError());
-            e->feat_seq[1] += m;
-            e->unsynced_records += m;
-            e->st.dns_ingested += m;
-        }
+        if (m) { if (int rc = fold_samples(e, 1, e->d_dnsc_out, m)) return rc; }
         e->st.dns_packets_ingested += c;
-        done += c;
+        in.advance(c);
     }
-    if (k != PTR_DEVICE) CU(cudaStreamSynchronize(e->copy_stream));
-    return FA_OK;
+    return in.finish(FA_OK, nullptr);
 }
 
 int fa_purge_stale_dns(fa_engine* e, uint64_t mono_now_ns, uint64_t timeout_ns) {
