@@ -60,7 +60,7 @@ constexpr uint32_t kProbeLimit = 8192;
 
 struct __align__(128) TeamSmem {                  // 26,496 B per team (128-record tiles)
     uint4    tile[kTile * kRecChunks];            // 18,432 B  one TMA-staged tile of records
-    uint32_t acc[kTile][8];                       //  4,096 B  per record: bytes lo / hi | packets | flags + duplicates << 16 | ns lo | end lo | ns hi | end hi
+    uint32_t acc[kTile][8];                       //  4,096 B  per record: bytes lo / hi | packets | flags + duplicates << 16 (+ kSketch packet carries << 24) | ns lo | end lo | ns hi | end hi
     uint32_t hs[kTile];                           //    512 B  low 32 bits of the slot hash
     uint4    res4[kTile];                         //  2,048 B  per representative: table slot | start mirror lo | eth + mirror hi | flag bits the hot line holds
     uint32_t rep[kRepSlots];                      //  1,024 B  tile-local election set: 23 hash bits << 8 | representative index
@@ -74,7 +74,7 @@ struct __align__(16) TeamCtl {                    // kept outside TeamSmem so th
 };
 struct __align__(16) HotEntry {                   // 208 B: a stride of 52 words keeps 8 entries on distinct banks
     uint4    line[8];                             // copy of the flow's identity line
-    uint32_t acc[8];                              // bytes lo/hi, packets, flags, ns lo (max), end lo (max), hits, -
+    uint32_t acc[8];                              // bytes lo/hi, packets, flags, ns lo (max), end lo (max), hits, packet carries (kSketch)
     uint32_t state;                               // 0 empty, 1 being filled, 2 live
     uint32_t hash;                                // low 32 bits of the slot hash
     uint32_t slot;
@@ -122,7 +122,10 @@ __device__ __forceinline__ void reduce_to_hot(const Table& t, uint32_t slot, uin
 }
 
 // Fused sketches (new capability, no reference): count-min += packets, HyperLogLog register = max(rho).
-__device__ __forceinline__ void sketch_update(const SketchParams& sk, uint64_t premix, uint32_t packets) {
+// The tile and cache accumulators hold a flow's packets in 32 bits, like the flow table, while the count-min counters
+// are 64-bit sums of every record's packets: with kSketch a fold whose 32-bit add carries also counts the carry
+// (tile: bits 24..31 of acc[3], above the duplicate count; cache: acc[7]), and `packets` here is the 64-bit total.
+__device__ __forceinline__ void sketch_update(const SketchParams& sk, uint64_t premix, uint64_t packets) {
     const uint64_t a = cms_hash_a(premix, sk.seed), b = cms_hash_b(premix, sk.seed);
     for (uint32_t d = 0; d < sk.depth; d++)
         red_add_u64(sk.cms + ((size_t)d << sk.log2w) + cms_index(a, b, d, sk.log2w), packets);
@@ -299,7 +302,8 @@ aggregate_kernel(const uint4* __restrict__ recs, uint32_t n, Table t, uint64_t e
                         const uint32_t prev = atomicAdd(&A[0], b_lo);
                         const uint32_t hi_add = b_hi + ((prev + b_lo) < prev ? 1u : 0u);
                         if (hi_add) atomicAdd(&A[1], hi_add);
-                        atomicAdd(&A[2], r4.x);
+                        const uint32_t p_prev = atomicAdd(&A[2], r4.x);
+                        if (kSketch && p_prev + r4.x < p_prev) atomicAdd(&A[7], 1u);          // count-min carry
                         const uint32_t fl = r4.y >> 16;
                         if (fl & ~A[3]) atomicOr(&A[3], fl);
                         if (v_start && (uint32_t)v_ns > A[4]) atomicMax(&A[4], (uint32_t)v_ns);
@@ -349,7 +353,8 @@ aggregate_kernel(const uint4* __restrict__ recs, uint32_t n, Table t, uint64_t e
                             const uint32_t prev = atomicAdd(&A[0], b_lo);
                             const uint32_t hi_add = b_hi + ((prev + b_lo) < prev ? 1u : 0u);
                             if (hi_add) atomicAdd(&A[1], hi_add);
-                            atomicAdd(&A[2], r4.x);
+                            const uint32_t p_prev = atomicAdd(&A[2], r4.x);
+                            if (kSketch && p_prev + r4.x < p_prev) atomicAdd(&A[3], 1u << 24);   // count-min carry
                             const uint32_t fl = r4.y >> 16;
                             if (fl) atomicOr(&A[3], fl);
                             if (v_start) atomicMax(&A[4], (uint32_t)v_ns);
@@ -507,7 +512,7 @@ aggregate_kernel(const uint4* __restrict__ recs, uint32_t n, Table t, uint64_t e
                 const uint4 a1 = *reinterpret_cast<const uint4*>(&s.acc[my_ridx][4]);
                 const uint64_t t_bytes = u64_of(a0.x, a0.y);
                 const uint32_t t_packets = a0.z;
-                const uint32_t t_flags = a0.w & 0xFFFFu, n_dups = a0.w >> 16;
+                const uint32_t t_flags = a0.w & 0xFFFFu, n_dups = kSketch ? (a0.w >> 16) & 0xFFu : a0.w >> 16;
                 const uint64_t t_ns = u64_of(a1.x, a1.z), t_end = u64_of(a1.y, a1.w);
                 const uint64_t v_ns = t_ns, v_end = t_end;           // the cache entry's windows: high words only
                 // a flow that shows up several times in one tile is hot: give it a cache entry if one is free
@@ -531,7 +536,7 @@ aggregate_kernel(const uint4* __restrict__ recs, uint32_t n, Table t, uint64_t e
                 if (kSketch) {
                     const uint4 r0 = R[0], r1 = R[1], k2 = R[2];
                     sketch_update(sk, key_premix(u64_of(r0.x, r0.y), u64_of(r0.z, r0.w), u64_of(r1.x, r1.y),
-                                                 u64_of(r1.z, r1.w), u64_of(k2.x, k2.y)), t_packets);
+                                                 u64_of(r1.z, r1.w), u64_of(k2.x, k2.y)), u64_of(t_packets, a0.w >> 24));
                 }
                 if (my_slot != kResSpill) {
                     reduce_to_hot(t, my_slot, t_bytes, t_packets, t_ns, t_end, t_flags, floor_ns, seen);
@@ -593,7 +598,7 @@ aggregate_kernel(const uint4* __restrict__ recs, uint32_t n, Table t, uint64_t e
             if (kSketch) {
                 const uint4 k0 = ce.line[0], k1 = ce.line[1], k2 = ce.line[2];
                 sketch_update(sk, key_premix(u64_of(k0.x, k0.y), u64_of(k0.z, k0.w), u64_of(k1.x, k1.y),
-                                             u64_of(k1.z, k1.w), u64_of(k2.x, k2.y)), A[2]);
+                                             u64_of(k1.z, k1.w), u64_of(k2.x, k2.y)), u64_of(A[2], A[7]));
             }
         }
     }
