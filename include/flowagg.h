@@ -384,6 +384,28 @@ typedef struct fa_evict_out {
 } fa_evict_out;
 int fa_evict_ex(fa_engine* e, const fa_evict_out* out, size_t cap, size_t* n_out);
 
+/* Top talkers of the current window: the min(k, live) live flows with the largest byte (FA_TOP_BYTES) or packet
+ * (FA_TOP_PACKETS) count, ranked on the device, WITHOUT removing or changing anything (table, feature lines, counters
+ * and live flow count are as before; a later eviction returns what it would have returned without the call).
+ *   Metric: the field as fa_evict_ex returns it: bytes (record offset 56) or packets (offset 64; wraps mod 2^32 in
+ *           ACCOUNTER mode; in KERNEL_MAP mode only packets of the first-seen interface).  Feature-only flows have 0.
+ *   Order:  metric descending; ties by ascending slot hash (fmix64(key_premix(key)), DESIGN.md §4), then by ascending
+ *           key bytes (memcmp over the 40 bytes).  Independent of slot position, table size, insertion order and mode.
+ *   Output: the blocks of `out` as in fa_evict_ex (host or device memory; `records` required, others may be NULL),
+ *           each with room for k rows; row i of every block is bit-identical to the row fa_evict_ex would return for
+ *           that flow now (feature blocks and the base patch included).  A requested block the engine does not produce
+ *           comes back zero.  *n_out = min(k, live); rows past it are not written.
+ *   Runs on the engine stream after every queued fold, under the engine lock, and returns when the outputs are
+ *   complete.  FA_F_NONBLOCKING_EVICT: ranks the live table only, not a retired table still being evicted.  The
+ *   fallback ring (fa_read_spilled) is not part of the table.  Device scratch O(k), allocated on first use.
+ *   FA_E_INVAL: null engine / out / out->records / n_out, unknown `by`, k == 0 or k > FA_TOP_MAX_K (nothing changes).
+ *   FA_E_CUDA: also when more than 4096 live flows share the k-th flow's metric value and 64-bit key premix (keys
+ *   built to collide on purpose; the table's probe chains would be as long). */
+#define FA_TOP_BYTES    0u
+#define FA_TOP_PACKETS  1u
+#define FA_TOP_MAX_K    (1u << 20)
+int fa_top_flows(fa_engine* e, uint32_t by, size_t k, const fa_evict_out* out, size_t* n_out);
+
 /* Lookup-and-RESET (no reference analogue; building block of the multi-GPU local combiner, the counterpart of
  * the reference folding its per-CPU maps in user space, pkg/tracer/tracer.go:1159-1187): every flow that received
  * records since the previous drain is written to out_records (device memory, cap x 144 B) as a partial flow record

@@ -10,6 +10,7 @@ FA_E_INVAL, FA_E_NOMEM, FA_E_CUDA, FA_E_NODEV, FA_E_2BIG, FA_E_CLOSED = -22, -12
 FA_MODE_ACCOUNTER, FA_MODE_KERNEL_MAP = 0, 1
 FA_F_ENABLE_RTT, FA_F_ENABLE_DNS, FA_F_ENABLE_SKETCH, FA_F_NO_FULL_CUT, FA_F_RINGBUF_FALLBACK, FA_F_ENABLE_PKT_DROP = 1, 2, 4, 8, 16, 32
 FA_F_NONBLOCKING_EVICT = 64
+FA_TOP_BYTES, FA_TOP_PACKETS, FA_TOP_MAX_K = 0, 1, 1 << 20
 FA_GEN_UNIFORM, FA_GEN_ZIPF = 0, 1
 FA_ABI_VERSION = 1
 
@@ -78,6 +79,7 @@ SIGNATURES = {
     "fa_ingest_dns_packets": (C.c_int, [C.c_void_p, C.c_void_p, C.c_size_t]),
     "fa_ingest_pkt_drops": (C.c_int, [C.c_void_p, C.c_void_p, C.c_size_t]),
     "fa_evict_ex": (C.c_int, [C.c_void_p, C.POINTER(EvictOut), C.c_size_t, C.POINTER(C.c_size_t)]),
+    "fa_top_flows": (C.c_int, [C.c_void_p, C.c_uint32, C.c_size_t, C.POINTER(EvictOut), C.POINTER(C.c_size_t)]),
     "fa_evict": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_size_t,
                            C.POINTER(C.c_size_t)]),
     "fa_drain_active": (C.c_int, [C.c_void_p, C.c_void_p, C.c_size_t, C.POINTER(C.c_size_t)]),

@@ -137,6 +137,16 @@ FA_HD uint32_t diff4_masked(uint4 a, uint4 b, uint4 m) {
 #define FA_EMUL_COUNT(which, n) ((void)0)
 #endif
 
+// A kernel launch written once for the device and the host emulation of the tests.  The emulation runs every CUDA
+// thread as an OS thread, so it caps the grid at 2 CTAs: only kernels whose loops are grid-stride may be launched this
+// way.  Dynamic shared memory is handed out per CTA (FA_DYN_SMEM).
+#ifdef FA_HOST_EMUL
+#define FA_LAUNCH(kernel, grid, block, smem, st, ...) \
+    simt::launch((unsigned)(grid) < 2u ? (unsigned)(grid) : 2u, (block), (smem), [=] { kernel(__VA_ARGS__); })
+#else
+#define FA_LAUNCH(kernel, grid, block, smem, st, ...) kernel<<<(grid), (block), (smem), (st)>>>(__VA_ARGS__)
+#endif
+
 #ifdef __CUDACC__
 // ------------------------------------------------------------------ PTX helpers
 __device__ __forceinline__ uint32_t smem_u32(const void* p) { return (uint32_t)__cvta_generic_to_shared(p); }

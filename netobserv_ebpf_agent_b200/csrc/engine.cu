@@ -142,12 +142,18 @@ struct fa_engine {
     uint32_t* d_snap_cnt = nullptr;           // ... records per CTA of the parse kernels, then the total + 3 filter counters (u64)
     uint8_t* d_snap_verdict = nullptr;        // ... with a flow filter: keep / skip per snapshot of the chunk
     fa::FilterSet filter{};                   // fa_set_flow_filter (n_rules == 0: no filter)
-    uint8_t* d_evict = nullptr; uint64_t evict_cap = 0;
-    uint8_t* d_evict_dns = nullptr; uint8_t* d_evict_add = nullptr; uint8_t* d_evict_present = nullptr;
-    uint32_t* d_slot_of_out = nullptr; uint64_t feat_evict_cap = 0;
+    // device staging of the host-bound fa_evict_ex blocks and the feature pass's slot list, grown on demand
+    struct Staging {
+        uint8_t* rec = nullptr; uint64_t cap = 0;
+        uint8_t *dns = nullptr, *add = nullptr, *drop = nullptr, *present = nullptr;
+        unsigned long long* rttmin = nullptr; uint32_t* slot_of = nullptr; uint64_t feat_cap = 0;
+    };
+    Staging evict_stage;                      // eviction: under `mu` (blocking) or `evict_mu` alone (non-blocking)
+    Staging top_stage;                        // fa_top_flows: under `mu`
+    fa::TopScratch top{};                     // fa_top_flows select state, histograms and candidates (cap entries)
+    fa::TopState* h_top_state = nullptr;      // pinned
     uint32_t* d_slot_of = nullptr;            // per-sample slot scratch of the feature folds
     uint64_t feat_seq[3] = {0, 0, 0};         // running sample numbers (additional, dns, packet drops)
-    uint8_t* d_evict_drop = nullptr; unsigned long long* d_evict_rttmin = nullptr;
     uint32_t* d_route_tmp = nullptr; unsigned long long* d_route_counts = nullptr;
 
     fa::SketchParams sk{};
@@ -482,6 +488,12 @@ static int alloc_table(fa_engine* e, fa::Table* t) {
     return FA_OK;
 }
 
+static void free_staging(fa_engine::Staging* s) {
+    cudaFree(s->rec); cudaFree(s->dns); cudaFree(s->add); cudaFree(s->drop); cudaFree(s->present);
+    cudaFree(s->rttmin); cudaFree(s->slot_of);
+    *s = fa_engine::Staging{};
+}
+
 static void free_table(fa::Table* t) {
     cudaFree(t->ident); cudaFree(t->hot); cudaFree(t->met); cudaFree(t->occ);
     cudaFree(t->feat_add); cudaFree(t->feat_dns); cudaFree(t->feat_drop);
@@ -659,10 +671,10 @@ void fa_destroy(fa_engine* e) {
     }
     cudaFree(e->d_scratch); cudaFree(e->d_spill_idx); cudaFree(e->d_cut_set); cudaFree(e->d_cut_bitmap); cudaFree(e->d_cut_out);
     if (e->h_cut_out) cudaFreeHost(e->h_cut_out);
-    cudaFree(e->d_evict); cudaFree(e->d_route_tmp); cudaFree(e->d_route_counts); cudaFree(e->d_expanded);
+    cudaFree(e->d_route_tmp); cudaFree(e->d_route_counts); cudaFree(e->d_expanded);
     cudaFree(e->d_snap_src); cudaFree(e->d_snap_cnt); cudaFree(e->d_snap_verdict);
-    cudaFree(e->d_evict_dns); cudaFree(e->d_evict_add); cudaFree(e->d_evict_present); cudaFree(e->d_slot_of_out); cudaFree(e->d_slot_of);
-    cudaFree(e->d_evict_drop); cudaFree(e->d_evict_rttmin);
+    free_staging(&e->evict_stage); free_staging(&e->top_stage); cudaFree(e->d_slot_of);
+    cudaFree(e->top.state); cudaFree(e->top.hist); cudaFree(e->top.ents); if (e->h_top_state) cudaFreeHost(e->h_top_state);
     cudaFree(e->sk.cms); cudaFree(e->sk.hll);
     cudaFree(e->dnsc.tab); cudaFree(e->dnsc_spare); cudaFree(e->dnsc.ctr); cudaFreeHost(e->h_dnsc_ctr);
     cudaFree(e->d_dnsc_state); cudaFree(e->d_dnsc_samples); cudaFree(e->d_dnsc_out); cudaFree(e->d_dnsc_warps);
@@ -870,77 +882,90 @@ int fa_live_flows(fa_engine* e, size_t* n) {
     return FA_OK;
 }
 
-// Device staging of the host-bound blocks of fa_evict_ex and the slot list of the feature pass, grown on demand.  Only
-// eviction touches it (the blocking path under `mu`, the non-blocking one under `evict_mu` alone), never fa_ingest*.
-static int evict_staging(fa_engine* e, uint64_t live, bool records, bool feats) {
-    const uint64_t want = std::max<uint64_t>(live, std::min<uint64_t>(e->cfg.max_entries, live * 2));
-    if (records && e->evict_cap < live) {
-        cudaFree(e->d_evict); e->d_evict = nullptr; e->evict_cap = 0;
-        CU(cudaMalloc(&e->d_evict, want * fa::kRecBytes));
-        e->evict_cap = want;
+// Device staging of the host-bound blocks of fa_evict_ex / fa_top_flows and the slot list of the feature pass, grown
+// on demand to hold n rows.  Eviction and fa_top_flows each have their own, never touched by fa_ingest*.
+static int grow_staging(fa_engine* e, fa_engine::Staging* s, uint64_t n, bool records, bool feats) {
+    const uint64_t want = std::max<uint64_t>(n, std::min<uint64_t>(e->cfg.max_entries, n * 2));
+    if (records && s->cap < n) {
+        cudaFree(s->rec); s->rec = nullptr; s->cap = 0;
+        CU(cudaMalloc(&s->rec, want * fa::kRecBytes));
+        s->cap = want;
     }
-    if (feats && e->feat_evict_cap < live) {
-        cudaFree(e->d_evict_dns); cudaFree(e->d_evict_add); cudaFree(e->d_evict_present); cudaFree(e->d_slot_of_out);
-        cudaFree(e->d_evict_drop); cudaFree(e->d_evict_rttmin);
-        e->d_evict_dns = e->d_evict_add = e->d_evict_present = e->d_evict_drop = nullptr; e->d_evict_rttmin = nullptr;
-        e->d_slot_of_out = nullptr; e->feat_evict_cap = 0;
-        CU(cudaMalloc(&e->d_evict_dns, want * 64)); CU(cudaMalloc(&e->d_evict_add, want * 32));
-        CU(cudaMalloc(&e->d_evict_drop, want * 32)); CU(cudaMalloc(&e->d_evict_rttmin, want * 8));
-        CU(cudaMalloc(&e->d_evict_present, want)); CU(cudaMalloc(&e->d_slot_of_out, want * 4));
-        e->feat_evict_cap = want;
+    if (feats && s->feat_cap < n) {
+        cudaFree(s->dns); cudaFree(s->add); cudaFree(s->present); cudaFree(s->slot_of); cudaFree(s->drop); cudaFree(s->rttmin);
+        s->dns = s->add = s->present = s->drop = nullptr; s->rttmin = nullptr; s->slot_of = nullptr; s->feat_cap = 0;
+        CU(cudaMalloc(&s->dns, want * 64)); CU(cudaMalloc(&s->add, want * 32));
+        CU(cudaMalloc(&s->drop, want * 32)); CU(cudaMalloc(&s->rttmin, want * 8));
+        CU(cudaMalloc(&s->present, want)); CU(cudaMalloc(&s->slot_of, want * 4));
+        s->feat_cap = want;
     }
     return FA_OK;
 }
 
-// Lookup-and-delete the `live` flows of `t` into the blocks of `o`, on stream `st`: the table scan (K2, or the
-// KERNEL_MAP scan) with ctr->evict_out as its cursor, the feature pass when `t` has feature lines, then the copies of
-// the blocks that are host memory (device blocks are written in place; staging from evict_staging).  Every requested
-// block the table does not produce comes out zero, whichever memory it is in.  Adds the kernels launched and the bytes
-// copied.
-static int evict_scan(fa_engine* e, const fa::Table& t, const fa_evict_out* o, uint64_t live, fa::Counters* ctr,
-                      cudaStream_t st, uint64_t* launches, uint64_t* d2h) {
+// Where the kernels write the n rows of each block of `o` for table `t`: device blocks in place, host blocks in the
+// staging `s` (grown by grow_staging).  Every requested block the table does not produce is zeroed where it lives.
+struct Blocks { uint8_t *rec, *dns, *add, *drop, *rmin, *pres; uint32_t* slot_of; };
+static int place_blocks(const fa::Table& t, const fa_evict_out* o, uint64_t n, const fa_engine::Staging& s, cudaStream_t st,
+                        Blocks* d) {
     const bool feats = t.feat_add || t.feat_dns || t.feat_drop;
     auto dev = [](void* p, void* staging) -> uint8_t* {          // where the kernels write a block
         return static_cast<uint8_t*>(p && classify(p) != PTR_DEVICE ? staging : p);
     };
-    uint8_t* d_out = dev(o->records, e->d_evict);
-    uint8_t *d_dns = nullptr, *d_add = nullptr, *d_drop = nullptr, *d_rmin = nullptr, *d_pres = nullptr;
+    *d = Blocks{};
+    d->rec = dev(o->records, s.rec);
     if (feats) {
-        d_dns = dev(o->dns, e->d_evict_dns); d_add = dev(o->additional, e->d_evict_add); d_drop = dev(o->pkt_drops, e->d_evict_drop);
-        d_rmin = dev(o->rtt_min, e->d_evict_rttmin); d_pres = dev(o->present, e->d_evict_present);
+        d->dns = dev(o->dns, s.dns); d->add = dev(o->additional, s.add); d->drop = dev(o->pkt_drops, s.drop);
+        d->rmin = dev(o->rtt_min, s.rttmin); d->pres = dev(o->present, s.present);
+        d->slot_of = s.slot_of;
         // the block of a feature this engine does not fold is zeroed where the kernels write (the feature pass does not
         // write it) and copied like the others
-        if (d_dns && !t.feat_dns) CU(cudaMemsetAsync(d_dns, 0, live * 64, st));
-        if (d_add && !t.feat_add) CU(cudaMemsetAsync(d_add, 0, live * 32, st));
-        if (d_drop && !t.feat_drop) CU(cudaMemsetAsync(d_drop, 0, live * 32, st));
+        if (d->dns && !t.feat_dns) CU(cudaMemsetAsync(d->dns, 0, n * 64, st));
+        if (d->add && !t.feat_add) CU(cudaMemsetAsync(d->add, 0, n * 32, st));
+        if (d->drop && !t.feat_drop) CU(cudaMemsetAsync(d->drop, 0, n * 32, st));
     } else {
         // no feature pass: every feature block is zeroed where it is
         const struct { void* p; size_t width; } unmade[5] = {
             {o->dns, 64}, {o->additional, 32}, {o->pkt_drops, 32}, {o->rtt_min, 8}, {o->present, 1}};
         for (const auto& b : unmade) {
             if (!b.p) continue;
-            if (classify(b.p) == PTR_DEVICE) CU(cudaMemsetAsync(b.p, 0, live * b.width, st));
-            else memset(b.p, 0, live * b.width);
+            if (classify(b.p) == PTR_DEVICE) CU(cudaMemsetAsync(b.p, 0, n * b.width, st));
+            else memset(b.p, 0, n * b.width);
         }
     }
-    uint32_t* slot_of_out = feats ? e->d_slot_of_out : nullptr;
-    if (e->cfg.mode == FA_MODE_KERNEL_MAP)
-        *launches += fa::launch_kmap_evict(t, t.met, d_out, live, &ctr->evict_out, slot_of_out, e->sm_count, st);
-    else
-        *launches += fa::launch_evict(t, reinterpret_cast<uint4*>(d_out), slot_of_out, live, ctr, e->sm_count, st);
-    if (feats)
-        *launches += fa::launch_evict_features(t, slot_of_out, live, d_out, d_dns, d_add, d_drop,
-                                               reinterpret_cast<unsigned long long*>(d_rmin), d_pres, e->sm_count, st);
+    return FA_OK;
+}
+
+// After the kernels: the feature pass over the n rows (when `t` has feature lines; clear = false leaves them as they
+// are), then the copies of the blocks that are host memory.  Adds the kernels launched and the bytes copied.
+static int finish_blocks(fa_engine* e, const fa::Table& t, const fa_evict_out* o, uint64_t n, const Blocks& d, bool clear,
+                         cudaStream_t st, uint64_t* launches, uint64_t* d2h) {
+    if (t.feat_add || t.feat_dns || t.feat_drop)
+        *launches += (clear ? fa::launch_evict_features : fa::launch_peek_features)(
+            t, d.slot_of, n, d.rec, d.dns, d.add, d.drop, reinterpret_cast<unsigned long long*>(d.rmin), d.pres, e->sm_count, st);
     CU(cudaGetLastError());
     const struct { void* host; const uint8_t* src; size_t width; } blocks[6] = {
-        {o->records, d_out, fa::kRecBytes}, {o->dns, d_dns, 64}, {o->additional, d_add, 32}, {o->pkt_drops, d_drop, 32},
-        {o->rtt_min, d_rmin, 8}, {o->present, d_pres, 1}};
+        {o->records, d.rec, fa::kRecBytes}, {o->dns, d.dns, 64}, {o->additional, d.add, 32}, {o->pkt_drops, d.drop, 32},
+        {o->rtt_min, d.rmin, 8}, {o->present, d.pres, 1}};
     for (const auto& b : blocks) {
         if (!b.host || !b.src || b.src == b.host) continue;        // not asked for, not produced, or written in place
-        CU(cudaMemcpyAsync(b.host, b.src, live * b.width, cudaMemcpyDeviceToHost, st));
-        *d2h += live * b.width;
+        CU(cudaMemcpyAsync(b.host, b.src, n * b.width, cudaMemcpyDeviceToHost, st));
+        *d2h += n * b.width;
     }
     return FA_OK;
+}
+
+// Lookup-and-delete the `live` flows of `t` into the blocks of `o`, on stream `st`: the table scan (K2, or the
+// KERNEL_MAP scan) with ctr->evict_out as its cursor, the feature pass when `t` has feature lines, then the copies of
+// the blocks that are host memory.  Adds the kernels launched and the bytes copied.
+static int evict_scan(fa_engine* e, const fa::Table& t, const fa_evict_out* o, uint64_t live, fa::Counters* ctr,
+                      cudaStream_t st, uint64_t* launches, uint64_t* d2h) {
+    Blocks d;
+    if (int rc = place_blocks(t, o, live, e->evict_stage, st, &d)) return rc;
+    if (e->cfg.mode == FA_MODE_KERNEL_MAP)
+        *launches += fa::launch_kmap_evict(t, t.met, d.rec, live, &ctr->evict_out, d.slot_of, e->sm_count, st);
+    else
+        *launches += fa::launch_evict(t, reinterpret_cast<uint4*>(d.rec), d.slot_of, live, ctr, e->sm_count, st);
+    return finish_blocks(e, t, o, live, d, /*clear=*/true, st, launches, d2h);
 }
 
 // Lookup-and-delete every flow.  Blocking: the live table is scanned on the engine stream under `mu`.
@@ -976,7 +1001,7 @@ int fa_evict_ex(fa_engine* e, const fa_evict_out* o, size_t cap, size_t* n_out) 
         st = e->evict_stream;
     }
     const bool feats = t.feat_add || t.feat_dns || t.feat_drop;
-    if (int rc = evict_staging(e, live, classify(o->records) != PTR_DEVICE, feats)) return rc;
+    if (int rc = grow_staging(e, &e->evict_stage, live, classify(o->records) != PTR_DEVICE, feats)) return rc;
     if (swap) CU(cudaStreamWaitEvent(st, e->ev_swap, 0));
     CU(cudaMemsetAsync(&ctr->evict_out, 0, sizeof(unsigned long long), st));
     uint64_t launched = 0, d2h = 0;
@@ -1009,6 +1034,65 @@ int fa_evict(fa_engine* e, void* out_records, void* out_dns, void* out_additiona
     fa_evict_out o{};
     o.records = out_records; o.dns = out_dns; o.additional = out_additional; o.present = out_present;
     return fa_evict_ex(e, &o, cap, n_out);
+}
+
+// The exact top-k live flows by bytes or packets, read in place (evict.cu: launch_top_flows).  The select, the
+// compaction, the sort and the gather run on the engine stream after the queued folds; the feature pass runs with
+// clear = false.  Nothing of the table or the counters is written.
+int fa_top_flows(fa_engine* e, uint32_t by, size_t k, const fa_evict_out* o, size_t* n_out) {
+    if (n_out) *n_out = 0;
+    if (!e || !o || !o->records || !n_out) return fail(FA_E_INVAL, "fa_top_flows: null argument");
+    if (by != FA_TOP_BYTES && by != FA_TOP_PACKETS) return fail(FA_E_INVAL, "fa_top_flows: unknown metric %u", by);
+    if (k == 0 || k > FA_TOP_MAX_K) return fail(FA_E_INVAL, "fa_top_flows: k = %zu not in [1, %u]", k, FA_TOP_MAX_K);
+    std::lock_guard<std::mutex> lk(e->mu);
+    CU(cudaSetDevice(e->device));
+    if (int rc = sync_counters(e)) return rc;          // the queued folds finish; exact live count
+    const uint64_t live = e->live_known;
+    const uint64_t n = std::min<uint64_t>(k, live);
+    if (n == 0) return FA_OK;
+    const fa::Table t = e->table;
+    const bool kmap = e->cfg.mode == FA_MODE_KERNEL_MAP;
+    const bool feats = t.feat_add || t.feat_dns || t.feat_drop;
+    cudaStream_t st = e->stream;
+    // FA_TOP_SLACK (diagnostics, tests): the room beyond k; a small one makes small tables run the digit passes
+    uint64_t slack = fa::kTopSlack;
+    if (const char* ts = getenv("FA_TOP_SLACK")) slack = strtoull(ts, nullptr, 0);
+    uint64_t cap = fa::kTopSortTile;
+    while (cap < n + slack) cap <<= 1;
+    if (e->top.cap < cap) {
+        cudaFree(e->top.ents); e->top.ents = nullptr; e->top.cap = 0;
+        CU(cudaMalloc(&e->top.ents, cap * sizeof(fa::TopEnt)));
+        e->top.cap = cap;
+    }
+    if (!e->top.state) {
+        CU(cudaMalloc(&e->top.state, sizeof(fa::TopState)));
+        CU(cudaMalloc(&e->top.hist, fa::kTopPasses * 256 * sizeof(unsigned)));
+        CU(cudaHostAlloc(&e->h_top_state, sizeof(fa::TopState), cudaHostAllocDefault));
+    }
+    fa::TopScratch s = e->top;
+    s.cap = cap;                                       // a larger scratch from an earlier call: sort only what is needed
+    if (int rc = grow_staging(e, &e->top_stage, n, classify(o->records) != PTR_DEVICE, feats)) return rc;
+    Blocks d;
+    if (int rc = place_blocks(t, o, n, e->top_stage, st, &d)) return rc;
+    fa::TopMetric M{};
+    M.p = kmap ? t.met + (by == FA_TOP_BYTES ? fa::KM_BYTES : fa::KM_PACKETS) : reinterpret_cast<const uint8_t*>(t.hot) + (by == FA_TOP_BYTES ? 0 : 24);
+    M.stride = kmap ? fa::kMetLineBytes : fa::kHotBytes;
+    M.wide = by == FA_TOP_BYTES;
+    CU(cudaMemsetAsync(s.state, 0, sizeof(fa::TopState), st));
+    CU(cudaMemsetAsync(s.hist, 0, fa::kTopPasses * 256 * sizeof(unsigned), st));
+    uint64_t launched = 0, d2h = 0;
+    launched += fa::launch_top_flows(t, kmap, M, n, live, s, d.rec, d.slot_of, e->sm_count, st);
+    if (int rc = finish_blocks(e, t, o, n, d, /*clear=*/false, st, &launched, &d2h)) return rc;
+    CU(cudaMemcpyAsync(e->h_top_state, s.state, sizeof(fa::TopState), cudaMemcpyDeviceToHost, st));
+    CU(cudaStreamSynchronize(st));
+    if (e->h_top_state->overflow || e->h_top_state->count < n)
+        return fail(FA_E_CUDA, "fa_top_flows: %llu candidates for %llu rows in a scratch of %llu (more than %llu flows tie with the "
+                    "k-th in metric and key premix)", e->h_top_state->count, (unsigned long long)n, (unsigned long long)cap,
+                    (unsigned long long)(cap - n));
+    e->st.kernel_launches += launched;
+    e->st.d2h_bytes += d2h;
+    *n_out = (size_t)n;
+    return FA_OK;
 }
 
 // Emit and reset the flows touched since the last drain into out_records_dev.  The count goes to *n_dev_out (device

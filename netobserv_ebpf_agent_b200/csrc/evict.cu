@@ -8,8 +8,35 @@
 // 144-byte record (9 x 16-byte stores), one output-cursor atomic per 32 slots, and in-place
 // clearing so the table comes out empty.
 #include "kernels.cuh"
+#include "kmap_body.cuh"
 
 namespace fa {
+
+// The 8 lanes of group g (lane j of the group) assemble the 144-byte record of `slot` from its identity line and hot
+// line, and store it at O (9 x 16-byte stores) when `store`.  Every lane of the warp calls it (the hot-line words
+// travel by shuffle); live = false for a group without a flow.  Shared by K2 and the fa_top_flows gather.
+__device__ __forceinline__ void emit_record(const Table& t, uint64_t slot, bool live, bool store, uint4* O, int g, int j) {
+    uint4 line = make_uint4(0, 0, 0, 0), hot = make_uint4(0, 0, 0, 0);
+    if (live) line = ld_cg_u4(&t.ident[slot * 8 + j]);
+    if (live && j < 2) hot = ld_cg_u4(&t.hot[slot * 2 + j]);
+    // hot chunk 0 = (bytes, nstart), hot chunk 1 = (end, packets, flags)
+    const uint32_t b_lo = __shfl_sync(0xFFFFFFFFu, hot.x, g * 8), b_hi = __shfl_sync(0xFFFFFFFFu, hot.y, g * 8);
+    const uint32_t ns_lo = __shfl_sync(0xFFFFFFFFu, hot.z, g * 8), ns_hi = __shfl_sync(0xFFFFFFFFu, hot.w, g * 8);
+    const uint32_t e_lo = __shfl_sync(0xFFFFFFFFu, hot.x, g * 8 + 1), e_hi = __shfl_sync(0xFFFFFFFFu, hot.y, g * 8 + 1);
+    const uint32_t pk = __shfl_sync(0xFFFFFFFFu, hot.z, g * 8 + 1), fl = __shfl_sync(0xFFFFFFFFu, hot.w, g * 8 + 1);
+    if (!store) return;
+    const uint64_t start = 0ull - u64_of(ns_lo, ns_hi);       // nstart = -start; 0 stays 0
+    if (j < 2) {
+        O[j] = line;                                            // key[0..32)
+    } else if (j == 2) {
+        O[2] = make_uint4(line.x, line.y & 0x00FFFFFFu, (uint32_t)start, (uint32_t)(start >> 32));
+    } else if (j == 3) {
+        O[3] = make_uint4(e_lo, e_hi, b_lo, b_hi);              // end, bytes
+        O[4] = make_uint4(pk, (line.y & 0xFFFFu) | (fl << 16), line.z, line.w);   // packets, eth|flags, desc[0..8)
+    } else {
+        O[j + 1] = line;                                        // desc[8..72)
+    }
+}
 
 // kDrain = false: lookup-and-delete (the flow is removed).  kDrain = true: "lookup-and-reset": flows that
 // received records since the last drain are emitted and their hot line is zeroed, but they stay in the table
@@ -73,34 +100,250 @@ evict_kernel(Table t, uint4* __restrict__ out, uint32_t* __restrict__ slot_of_ou
                 const uint32_t pos = live ? __fns(sbits, 0, within + 1) : 0u;
                 const uint64_t slot = (w0 + src) * 32 + pos;
                 const unsigned long long idx = base + f;
-                uint4 line = make_uint4(0, 0, 0, 0), hot = make_uint4(0, 0, 0, 0);
-                if (live) line = ld_cg_u4(&t.ident[slot * 8 + j]);
-                if (live && j < 2) hot = ld_cg_u4(&t.hot[slot * 2 + j]);
-                // hot chunk 0 = (bytes, nstart), hot chunk 1 = (end, packets, flags)
-                const uint32_t b_lo = __shfl_sync(0xFFFFFFFFu, hot.x, g * 8), b_hi = __shfl_sync(0xFFFFFFFFu, hot.y, g * 8);
-                const uint32_t ns_lo = __shfl_sync(0xFFFFFFFFu, hot.z, g * 8), ns_hi = __shfl_sync(0xFFFFFFFFu, hot.w, g * 8);
-                const uint32_t e_lo = __shfl_sync(0xFFFFFFFFu, hot.x, g * 8 + 1), e_hi = __shfl_sync(0xFFFFFFFFu, hot.y, g * 8 + 1);
-                const uint32_t pk = __shfl_sync(0xFFFFFFFFu, hot.z, g * 8 + 1), fl = __shfl_sync(0xFFFFFFFFu, hot.w, g * 8 + 1);
-                if (live && idx < cap) {
-                    uint4* O = out + idx * kRecChunks;
-                    const uint64_t start = 0ull - u64_of(ns_lo, ns_hi);       // nstart = -start; 0 stays 0
-                    if (j < 2) {
-                        O[j] = line;                                            // key[0..32)
-                    } else if (j == 2) {
-                        O[2] = make_uint4(line.x, line.y & 0x00FFFFFFu, (uint32_t)start, (uint32_t)(start >> 32));
-                    } else if (j == 3) {
-                        O[3] = make_uint4(e_lo, e_hi, b_lo, b_hi);              // end, bytes
-                        O[4] = make_uint4(pk, (line.y & 0xFFFFu) | (fl << 16), line.z, line.w);   // packets, eth|flags, desc[0..8)
-                    } else {
-                        O[j + 1] = line;                                        // desc[8..72)
-                    }
-                    if (slot_of_out && j == 0) slot_of_out[idx] = (uint32_t)slot;   // for the feature pass
-                }
+                const bool store = live && idx < cap;
+                emit_record(t, slot, live, store, out + idx * kRecChunks, g, j);
+                if (store && slot_of_out && j == 0) slot_of_out[idx] = (uint32_t)slot;   // for the feature pass
                 // delete: tag -> EMPTY, hot line -> identity  (drain: hot line only)
                 if (!kDrain && live && j == 2) *reinterpret_cast<uint2*>(reinterpret_cast<uint8_t*>(&t.ident[slot * 8 + 2]) + 8) = make_uint2(0u, 0u);
                 if (live && j < 2) t.hot[slot * 2 + j] = make_uint4(0, 0, 0, 0);
             }
         }
+    }
+}
+
+
+// ---- fa_top_flows: the exact top-k of the live flows, without removing or changing anything ------------------------
+// Rank order: metric descending, then slot hash ascending, then key bytes ascending.  A radix select over the 128-bit
+// composite (metric, ~slot hash) in 8-bit digits, from the byte that holds the largest metric's top bit, finds the
+// bucket of the k-th flow; it stops as soon as every flow above the bucket plus the bucket fit the scratch (or every
+// bit is resolved).  Those flows are compacted, sorted by a bitonic network (key compare for equal hashes) and the
+// first k gathered.  Passes read the bitmap and the metric word of the live flows; the key, for the hash, only where
+// the metric bits are tied with the prefix.
+
+FA_HD uint64_t shr64(uint64_t x, uint32_t s) { return s >= 64 ? 0ull : x >> s; }
+FA_HD uint64_t bswap64(uint64_t x) {
+    x = ((x & 0x00FF00FF00FF00FFull) << 8) | ((x >> 8) & 0x00FF00FF00FF00FFull);
+    x = ((x & 0x0000FFFF0000FFFFull) << 16) | ((x >> 16) & 0x0000FFFF0000FFFFull);
+    return (x << 32) | (x >> 32);
+}
+FA_HD uint64_t top_metric(const TopMetric& M, uint64_t slot) {
+    const uint8_t* p = M.p + slot * M.stride;
+    return M.wide ? *reinterpret_cast<const uint64_t*>(p) : (uint64_t)*reinterpret_cast<const uint32_t*>(p);
+}
+FA_HD uint64_t top_hash(const Table& t, uint64_t slot) {
+    const uint64_t* L = reinterpret_cast<const uint64_t*>(t.ident) + slot * (kIdentBytes / 8);
+    return slot_hash(key_premix(L[0], L[1], L[2], L[3], L[4]));
+}
+// The composite's resolved bits [pos, 128) against the prefix: < 0 below, 0 equal, > 0 above.  ~hash goes to lo when it
+// had to be computed (the metric bits are all resolved and equal).
+FA_HD int top_cmp(const Table& t, uint64_t slot, uint64_t m, const TopState& S, uint64_t& lo, bool& have_lo) {
+    if (S.pos >= 64) {
+        const uint64_t a = shr64(m, S.pos - 64), b = shr64(S.pm, S.pos - 64);
+        return a < b ? -1 : a > b ? 1 : 0;
+    }
+    if (m != S.pm) return m < S.pm ? -1 : 1;
+    lo = ~top_hash(t, slot);
+    have_lo = true;
+    const uint64_t a = lo >> S.pos, b = S.plo >> S.pos;
+    return a < b ? -1 : a > b ? 1 : 0;
+}
+// a ranks strictly before b; the padding (kTopNoSlot) after every flow
+FA_HD bool top_before(const Table& t, const TopEnt& a, const TopEnt& b) {
+    if (a.slot == kTopNoSlot || b.slot == kTopNoSlot) return a.slot != kTopNoSlot && b.slot == kTopNoSlot;
+    if (a.m != b.m) return a.m > b.m;
+    if (a.h != b.h) return a.h < b.h;
+    const uint64_t* A = reinterpret_cast<const uint64_t*>(t.ident) + (uint64_t)a.slot * (kIdentBytes / 8);
+    const uint64_t* B = reinterpret_cast<const uint64_t*>(t.ident) + (uint64_t)b.slot * (kIdentBytes / 8);
+    for (int w = 0; w < 5; w++) {                          // identical premix: the 40 key bytes in memcmp order
+        const uint64_t keep = w == 4 ? 0x00FFFFFFFFFFFFFFull : ~0ull;
+        const uint64_t x = bswap64(A[w] & keep), y = bswap64(B[w] & keep);
+        if (x != y) return x < y;
+    }
+    return false;
+}
+
+// Every thread owns one bitmap word per grid-stride step (a warp: 1024 slots in one coalesced load) and walks its set
+// bits.  n_words and the stride are multiples of 32, so the lanes of a warp take the same number of steps.
+#define TOP_FOR_WORDS(t, w) \
+    for (uint64_t w = blockIdx.x * (uint64_t)blockDim.x + threadIdx.x; w < (((t).mask + 1) >> 5); w += (uint64_t)gridDim.x * blockDim.x)
+
+__global__ void __launch_bounds__(256) top_max_kernel(Table t, TopMetric M, TopState* st) {
+    unsigned long long mx = 0;
+    TOP_FOR_WORDS(t, w) {
+        for (uint32_t r = t.occ[w]; r; r &= r - 1) {
+            const uint64_t m = top_metric(M, w * 32 + (__ffs(r) - 1));
+            mx = m > mx ? m : mx;
+        }
+    }
+    const int lane = threadIdx.x & 31;
+#pragma unroll
+    for (int d = 16; d > 0; d >>= 1) {
+        const unsigned long long o = __shfl_sync(0xFFFFFFFFu, mx, lane ^ d);
+        mx = o > mx ? o : mx;
+    }
+    if (lane == 0 && mx) atomicMax(&st->m_max, mx);
+}
+
+// One thread.  hist == nullptr: the start (the digits above the largest metric are zero for every flow).  Otherwise fix
+// the digit of the pass: the bucket that holds the k_rem-th candidate, counted from the top.
+__global__ void top_resolve_kernel(TopState* st, const unsigned* hist, unsigned long long k, unsigned long long live,
+                                   unsigned long long cap) {
+    if (threadIdx.x != 0) return;
+    TopState S = *st;
+    if (!hist) {
+        const uint32_t bits = 64u - (uint32_t)__clzll((long long)S.m_max);
+        S.pos = 64u + 8u * ((bits + 7u) / 8u);
+        S.k_rem = k; S.n_cand = live; S.above = 0;
+        S.done = live <= cap ? 1u : 0u;
+    } else {
+        if (S.done) return;
+        const uint32_t p = S.pos - 8u;
+        unsigned long long cum = 0;
+        uint32_t b = 255;
+        for (; b > 0; b--) {
+            if (cum + hist[b] >= S.k_rem) break;
+            cum += hist[b];
+        }
+        S.above += cum; S.k_rem -= cum; S.n_cand = hist[b];
+        if (p >= 64) S.pm |= (unsigned long long)b << (p - 64); else S.plo |= (unsigned long long)b << p;
+        S.pos = p;
+        S.passes++;
+        if (S.above + S.n_cand <= cap) S.done = 1;
+        else if (p == 0) { S.done = 1; S.overflow = 1; }
+    }
+    *st = S;
+}
+
+// Histogram of the next digit over the flows that match the prefix (256 bins in shared memory).
+__global__ void __launch_bounds__(256) top_hist_kernel(Table t, TopMetric M, const TopState* st, unsigned* hist) {
+    FA_DYN_SMEM(smem);
+    unsigned* H = reinterpret_cast<unsigned*>(smem);
+    const TopState S = *st;
+    if (S.done) return;
+    for (int b = threadIdx.x; b < 256; b += blockDim.x) H[b] = 0u;
+    __syncthreads();
+    const uint32_t p = S.pos - 8u;
+    TOP_FOR_WORDS(t, w) {
+        for (uint32_t r = t.occ[w]; r; r &= r - 1) {
+            const uint64_t slot = w * 32 + (__ffs(r) - 1);
+            const uint64_t m = top_metric(M, slot);
+            uint64_t lo = 0;
+            bool have_lo = false;
+            if (top_cmp(t, slot, m, S, lo, have_lo) != 0) continue;
+            uint32_t d;
+            if (p >= 64) {
+                d = (uint32_t)(m >> (p - 64)) & 255u;
+            } else {
+                if (!have_lo) lo = ~top_hash(t, slot);
+                d = (uint32_t)(lo >> p) & 255u;
+            }
+            atomicAdd(&H[d], 1u);
+        }
+    }
+    __syncthreads();
+    for (int b = threadIdx.x; b < 256; b += blockDim.x)
+        if (H[b]) atomicAdd(&hist[b], H[b]);
+}
+
+// Every flow at or above the prefix into ents (one cursor atomic per warp step); their count is above + n_cand.
+__global__ void __launch_bounds__(256) top_compact_kernel(Table t, TopMetric M, TopState* st, TopEnt* ents, unsigned long long cap) {
+    const TopState S = *st;
+    const int lane = threadIdx.x & 31;
+    TOP_FOR_WORDS(t, w) {
+        const uint32_t bits = t.occ[w];
+        uint32_t take = 0;
+        for (uint32_t r = bits; r; r &= r - 1) {
+            const int b = __ffs(r) - 1;
+            const uint64_t slot = w * 32 + b;
+            uint64_t lo = 0;
+            bool have_lo = false;
+            if (top_cmp(t, slot, top_metric(M, slot), S, lo, have_lo) >= 0) take |= 1u << b;
+        }
+        const uint32_t cnt = __popc(take);
+        uint32_t incl = cnt;
+#pragma unroll
+        for (int d = 1; d < 32; d <<= 1) { const uint32_t v = __shfl_up_sync(0xFFFFFFFFu, incl, d); if (lane >= d) incl += v; }
+        const uint32_t total = __shfl_sync(0xFFFFFFFFu, incl, 31);
+        if (total == 0u) continue;
+        unsigned long long base = 0;
+        if (lane == 0) base = atomicAdd(&st->count, (unsigned long long)total);
+        base = __shfl_sync(0xFFFFFFFFu, base, 0);
+        unsigned long long at = base + incl - cnt;
+        for (uint32_t r = take; r; r &= r - 1, at++) {
+            const uint64_t slot = w * 32 + (__ffs(r) - 1);
+            if (at < cap) {
+                TopEnt E;
+                E.m = top_metric(M, slot); E.h = top_hash(t, slot); E.slot = (uint32_t)slot; E.pad = 0u;
+                ents[at] = E;
+            }
+        }
+    }
+}
+
+// Bitonic network over n (a power of two) entries, ascending in top_before order.  size == 0: sort each tile of
+// kTopSortTile entries in shared memory (entries past the compaction count become padding).  Otherwise the strides
+// below kTopSortTile of the merge of `size`.  kTopSortTile / 2 threads, one pair each per step.
+__global__ void __launch_bounds__(kTopSortTile / 2) top_sort_tile_kernel(Table t, TopEnt* e, const TopState* st, unsigned long long n,
+                                                                          unsigned long long size) {
+    FA_DYN_SMEM(smem);
+    TopEnt* S = reinterpret_cast<TopEnt*>(smem);
+    const unsigned long long count = st->count;
+    const uint32_t q = threadIdx.x;
+    for (unsigned long long base = (unsigned long long)blockIdx.x * kTopSortTile; base < n; base += (unsigned long long)gridDim.x * kTopSortTile) {
+        for (uint32_t i = q; i < (uint32_t)kTopSortTile; i += blockDim.x) {
+            if (size == 0 && base + i >= count) { TopEnt E; E.m = 0; E.h = 0; E.slot = kTopNoSlot; E.pad = 0; S[i] = E; }
+            else S[i] = e[base + i];
+        }
+        __syncthreads();
+        const unsigned long long s_lo = size ? size : 2, s_hi = size ? size : kTopSortTile;
+        for (unsigned long long s = s_lo; s <= s_hi; s <<= 1) {
+            for (uint32_t j = (uint32_t)(s < (unsigned long long)kTopSortTile ? s : kTopSortTile) / 2; j > 0; j >>= 1) {
+                const uint32_t i = 2 * j * (q / j) + (q % j), l = i + j;
+                const bool up = ((base + i) & s) == 0;
+                const TopEnt a = S[i], b = S[l];
+                if (up ? top_before(t, b, a) : top_before(t, a, b)) { S[i] = b; S[l] = a; }
+                __syncthreads();
+            }
+        }
+        for (uint32_t i = q; i < (uint32_t)kTopSortTile; i += blockDim.x) e[base + i] = S[i];
+        __syncthreads();
+    }
+}
+// one step of the merge of `size` at stride j >= kTopSortTile, in global memory
+__global__ void __launch_bounds__(256) top_merge_kernel(Table t, TopEnt* e, unsigned long long n, unsigned long long size,
+                                                        unsigned long long j) {
+    for (unsigned long long q = blockIdx.x * (unsigned long long)blockDim.x + threadIdx.x; q < n / 2;
+         q += (unsigned long long)gridDim.x * blockDim.x) {
+        const unsigned long long i = 2 * j * (q / j) + (q % j), l = i + j;
+        const bool up = (i & size) == 0;
+        const TopEnt a = e[i], b = e[l];
+        if (up ? top_before(t, b, a) : top_before(t, a, b)) { e[i] = b; e[l] = a; }
+    }
+}
+
+// the first n sorted entries as records, ACCOUNTER layout (emit_record, 4 flows per warp step) ...
+__global__ void __launch_bounds__(256) top_gather_kernel(Table t, const TopEnt* __restrict__ e, unsigned long long n,
+                                                         uint4* __restrict__ out, uint32_t* __restrict__ slot_of_out) {
+    const int lane = threadIdx.x & 31, g = lane >> 3, j = lane & 7;
+    const unsigned long long warp_global = (blockIdx.x * (unsigned long long)blockDim.x + threadIdx.x) >> 5;
+    const unsigned long long n_warps = ((unsigned long long)gridDim.x * blockDim.x) >> 5;
+    for (unsigned long long f0 = warp_global * 4; f0 < n; f0 += n_warps * 4) {
+        const unsigned long long i = f0 + g;
+        const uint32_t s = i < n ? e[i].slot : kTopNoSlot;
+        const bool live = s != kTopNoSlot;                // padding in the first n: fewer candidates than n (the host
+        const uint64_t slot = live ? s : 0u;               // reports it); the row is left unwritten
+        emit_record(t, slot, live, live, out + i * kRecChunks, g, j);
+        if (slot_of_out && i < n && j == 0) slot_of_out[i] = (uint32_t)slot;   // padding: slot 0, read only by the peek
+    }
+}
+// ... and KERNEL_MAP layout (km_emit_record)
+__global__ void __launch_bounds__(256) top_gather_kmap_kernel(Table t, const TopEnt* __restrict__ e, unsigned long long n,
+                                                              uint8_t* __restrict__ out, uint32_t* __restrict__ slot_of_out) {
+    for (unsigned long long i = blockIdx.x * (unsigned long long)blockDim.x + threadIdx.x; i < n; i += (unsigned long long)gridDim.x * blockDim.x) {
+        const uint32_t slot = e[i].slot;
+        if (slot_of_out) slot_of_out[i] = slot == kTopNoSlot ? 0u : slot;   // padding: slot 0, read only by the peek
+        if (slot == kTopNoSlot) continue;                 // padding: fewer candidates than n (the host reports it)
+        km_emit_record(t, t.met, slot, out + i * kRecBytes);
     }
 }
 
@@ -112,5 +355,33 @@ int launch_evict(const Table& table, uint4* out_recs, uint32_t* slot_of_out,
     return 1;
 }
 #endif  // FA_HOST_EMUL
+
+// One text for the device and the host emulation (FA_LAUNCH): every kernel of the sequence loops grid-stride.
+int launch_top_flows(const Table& t, bool kmap, const TopMetric& M, uint64_t n, uint64_t live, const TopScratch& s,
+                     uint8_t* out_recs, uint32_t* slot_of_out, int sm_count, cudaStream_t st) {
+    const int grid = sm_count * 8;
+    const size_t tile_smem = kTopSortTile * sizeof(TopEnt);
+    int launches = 0;
+    FA_LAUNCH(top_max_kernel, grid, 256, 0, st, t, M, s.state);
+    FA_LAUNCH(top_resolve_kernel, 1, 32, 0, st, s.state, nullptr, n, live, s.cap);
+    for (int p = 0; p < kTopPasses; p++) {                 // fixed sequence: passes after the last needed one exit at once
+        FA_LAUNCH(top_hist_kernel, grid, 256, 256 * sizeof(unsigned), st, t, M, s.state, s.hist + p * 256);
+        FA_LAUNCH(top_resolve_kernel, 1, 32, 0, st, s.state, s.hist + p * 256, n, live, s.cap);
+    }
+    FA_LAUNCH(top_compact_kernel, grid, 256, 0, st, t, M, s.state, s.ents, s.cap);
+    launches += 3 + 2 * kTopPasses;
+    const unsigned tiles = (unsigned)(s.cap / kTopSortTile);
+    FA_LAUNCH(top_sort_tile_kernel, tiles, kTopSortTile / 2, tile_smem, st, t, s.ents, s.state, s.cap, 0ull);
+    launches++;
+    for (unsigned long long size = 2 * kTopSortTile; size <= s.cap; size <<= 1) {
+        for (unsigned long long j = size / 2; j >= (unsigned long long)kTopSortTile; j >>= 1, launches++)
+            FA_LAUNCH(top_merge_kernel, grid, 256, 0, st, t, s.ents, s.cap, size, j);
+        FA_LAUNCH(top_sort_tile_kernel, tiles, kTopSortTile / 2, tile_smem, st, t, s.ents, s.state, s.cap, size);
+        launches++;
+    }
+    if (kmap) FA_LAUNCH(top_gather_kmap_kernel, grid, 256, 0, st, t, s.ents, n, out_recs, slot_of_out);
+    else FA_LAUNCH(top_gather_kernel, grid, 256, 0, st, t, s.ents, n, reinterpret_cast<uint4*>(out_recs), slot_of_out);
+    return launches + 1;
+}
 
 }  // namespace fa

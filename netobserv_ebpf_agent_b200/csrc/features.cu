@@ -406,6 +406,8 @@ __device__ __forceinline__ void build_base(uint64_t& bs, uint64_t& be, uint32_t&
     if (beth == 0 && neth != 0) beth = (uint32_t)(~neth) & 0xFFFFu;
 }
 
+// kClear = false: the fa_top_flows peek, which emits the same rows and leaves the feature lines as they are.
+template <bool kClear = true>
 __global__ void evict_features_kernel(Table t, const uint32_t* __restrict__ slot_of_out, unsigned long long n_out,
                                       uint8_t* __restrict__ out_recs, uint8_t* __restrict__ out_dns,
                                       uint8_t* __restrict__ out_add, uint8_t* __restrict__ out_drop,
@@ -435,8 +437,10 @@ __global__ void evict_features_kernel(Table t, const uint32_t* __restrict__ slot
                     for (int b = 0; b < 32; b++) D[31 + b] = Sb[80 + b];
                     D[63] = 0;
                 }
+if (kClear) {
 #pragma unroll
-                for (int c = 0; c < 16; c++) S[c] = 0ull;
+                    for (int c = 0; c < 16; c++) S[c] = 0ull;
+                }
             } else if (out_dns) {
                 for (int c = 0; c < 8; c++) reinterpret_cast<uint64_t*>(out_dns + i * 64)[c] = 0ull;
             }
@@ -458,8 +462,10 @@ __global__ void evict_features_kernel(Table t, const uint32_t* __restrict__ slot
                     *reinterpret_cast<uint16_t*>(D + 26) = *reinterpret_cast<const uint16_t*>(Sb + 44);              // first.eth
                     *reinterpret_cast<uint32_t*>(D + 28) = (uint32_t)(S[4] & 0xFFu);          // latest_state: last non-zero; padding
                 }
+if (kClear) {
 #pragma unroll
-                for (int c = 0; c < 12; c++) S[c] = 0ull;
+                    for (int c = 0; c < 12; c++) S[c] = 0ull;
+                }
             } else if (out_drop) {
                 for (int c = 0; c < 4; c++) reinterpret_cast<uint64_t*>(out_drop + i * 32)[c] = 0ull;
             }
@@ -482,8 +488,10 @@ __global__ void evict_features_kernel(Table t, const uint32_t* __restrict__ slot
                     A[30] = (uint8_t)(ip & 1u);
                     A[31] = 0;
                 }
+if (kClear) {
 #pragma unroll
-                for (int c = 0; c < 10; c++) S[c] = 0ull;
+                    for (int c = 0; c < 10; c++) S[c] = 0ull;
+                }
             } else if (out_add) {
                 for (int c = 0; c < 4; c++) reinterpret_cast<uint64_t*>(out_add + i * 32)[c] = 0ull;
             }
@@ -502,9 +510,18 @@ int launch_evict_features(const Table& t, const uint32_t* slot_of_out, unsigned 
                           uint8_t* out_dns, uint8_t* out_add, uint8_t* out_drop, unsigned long long* out_rtt_min,
                           uint8_t* out_present, int sm_count, cudaStream_t st) {
     if (!n_out) return 0;
-    evict_features_kernel<<<sm_count * 8, 256, 0, st>>>(t, slot_of_out, n_out, out_recs, out_dns, out_add, out_drop, out_rtt_min, out_present);
+    evict_features_kernel<true><<<sm_count * 8, 256, 0, st>>>(t, slot_of_out, n_out, out_recs, out_dns, out_add, out_drop, out_rtt_min, out_present);
     return 1;
 }
 #endif  // FA_HOST_EMUL
+
+int launch_peek_features(const Table& t, const uint32_t* slot_of_out, unsigned long long n_out, uint8_t* out_recs,
+                         uint8_t* out_dns, uint8_t* out_add, uint8_t* out_drop, unsigned long long* out_rtt_min,
+                         uint8_t* out_present, int sm_count, cudaStream_t st) {
+    if (!n_out) return 0;
+    FA_LAUNCH(evict_features_kernel<false>, sm_count * 8, 256, 0, st, t, slot_of_out, n_out, out_recs, out_dns, out_add, out_drop,
+              out_rtt_min, out_present);
+    return 1;
+}
 
 }  // namespace fa

@@ -65,6 +65,43 @@ int launch_feature_fold(int kind, const uint8_t* recs, uint32_t n, const Table& 
 int launch_evict_features(const Table& t, const uint32_t* slot_of_out, unsigned long long n_out, uint8_t* out_recs,
                           uint8_t* out_dns, uint8_t* out_add, uint8_t* out_drop, unsigned long long* out_rtt_min,
                           uint8_t* out_present, int sm_count, cudaStream_t st);
+// the same rows for fa_top_flows, leaving the feature lines as they are
+int launch_peek_features(const Table& t, const uint32_t* slot_of_out, unsigned long long n_out, uint8_t* out_recs,
+                         uint8_t* out_dns, uint8_t* out_add, uint8_t* out_drop, unsigned long long* out_rtt_min,
+                         uint8_t* out_present, int sm_count, cudaStream_t st);
+
+// fa_top_flows (evict.cu): radix select over the composite (metric, ~slot hash), compaction, sort, gather.
+// Where a flow's metric is: the u64 (wide) or u32 at p + slot * stride (the hot line or the KERNEL_MAP metric line).
+struct TopMetric { const uint8_t* p; uint32_t stride; uint32_t wide; };
+// one compacted candidate; slot == kTopNoSlot marks the padding that sorts last
+struct TopEnt { unsigned long long m, h; uint32_t slot, pad; };
+constexpr uint32_t kTopNoSlot = 0xFFFFFFFFu;
+constexpr int kTopPasses = 16;                     // 8-bit digits of the 128-bit composite; later passes exit at once
+constexpr int kTopSortTile = 1024;                 // entries sorted in shared memory by one CTA
+constexpr uint64_t kTopSlack = 4096;               // compaction room beyond k: the select stops once the candidates fit
+// select state, on the device: the composite's bits [pos, 128) are resolved to (pm, plo)
+struct TopState {
+    unsigned long long m_max;                      // largest metric (first kernel)
+    unsigned long long pm, plo;                    // resolved prefix: metric bits, ~hash bits
+    unsigned long long above;                      // flows strictly above the prefix (all of them are in the result)
+    unsigned long long k_rem;                      // result rows still to come from the flows that match the prefix
+    unsigned long long n_cand;                     // flows that match the prefix
+    unsigned long long count;                      // compaction cursor
+    uint32_t pos;                                  // lowest resolved bit
+    uint32_t done;                                 // 1: above + n_cand fit the scratch, or every bit is resolved
+    uint32_t overflow;                             // every bit resolved and still more candidates than scratch
+    uint32_t passes;                               // digit passes taken
+};
+struct TopScratch {
+    TopState* state;                               // zeroed before the launch (with hist)
+    unsigned* hist;                                // kTopPasses x 256
+    TopEnt* ents;                                  // cap entries (cap: power of two >= k + kTopSlack)
+    uint64_t cap;
+};
+// The n (<= live) highest-ranked live flows of `t` into out_recs (device, n x 144 B) in rank order, and their slots into
+// slot_of_out (optional, for the feature pass).  kmap: KERNEL_MAP record layout.  Nothing in `t` changes.
+int launch_top_flows(const Table& t, bool kmap, const TopMetric& M, uint64_t n, uint64_t live, const TopScratch& s,
+                     uint8_t* out_recs, uint32_t* slot_of_out, int sm_count, cudaStream_t st);
 
 // sketches
 int launch_cms_query(const SketchParams& sk, const uint4* keys, uint32_t n, unsigned long long* est, cudaStream_t st);

@@ -563,6 +563,15 @@ FA_HD void km2_finish_flow_body(const KmParams& P, uint32_t k) {
 }
 
 // ---- evict: one call per occupancy word (32 slots) -------------------------------------------------------------
+// the 144-byte record of `slot`: key (identity line) + flow_metrics (metric line).  Shared by the eviction and the
+// fa_top_flows gather (evict.cu).
+FA_HD void km_emit_record(const Table& t, const uint8_t* met, uint32_t slot, uint8_t* out_rec) {
+    const uint64_t* L = reinterpret_cast<const uint64_t*>(reinterpret_cast<const uint8_t*>(t.ident) + (size_t)slot * kIdentBytes);
+    const uint64_t* M = reinterpret_cast<const uint64_t*>(met + (size_t)slot * kMetLineBytes);
+    uint64_t* O = reinterpret_cast<uint64_t*>(out_rec);
+    for (int k = 0; k < 5; k++) O[k] = L[k];
+    for (int k = 0; k < 13; k++) O[5 + k] = M[k];
+}
 FA_HD void km_evict_word_body(const Table& t, uint8_t* met, uint32_t w, uint8_t* out, unsigned long long cap,
                               unsigned long long* cursor, uint32_t* slot_of_out = nullptr) {
     uint32_t bits = t.occ[w];
@@ -575,9 +584,7 @@ FA_HD void km_evict_word_body(const Table& t, uint8_t* met, uint32_t w, uint8_t*
         uint64_t* M = reinterpret_cast<uint64_t*>(met + (size_t)slot * kMetLineBytes);
         const unsigned long long at = km_add64(cursor, 1ull);
         if (at < cap) {
-            uint64_t* O = reinterpret_cast<uint64_t*>(out + (size_t)at * kRecBytes);
-            for (int k = 0; k < 5; k++) O[k] = L[k];
-            for (int k = 0; k < 13; k++) O[5 + k] = M[k];
+            km_emit_record(t, met, slot, out + (size_t)at * kRecBytes);
             if (slot_of_out) slot_of_out[at] = slot;                    // for the feature pass (evict_features_kernel)
         }
         for (int k = 0; k < 16; k++) { L[k] = 0ull; M[k] = 0ull; }

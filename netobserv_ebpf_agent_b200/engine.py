@@ -167,6 +167,22 @@ class FlowAggEngine:
         g = got.value
         return out[:g], dns[:g], add[:g], drops[:g], rmin[:g], pres[:g]
 
+    def top_flows(self, k, by="bytes"):
+        """The min(k, live) live flows with the most bytes (by="bytes") or packets (by="packets"), ranked, without
+        removing or changing anything -> the six arrays of evict_ex (records, dns, additional, pkt_drops, rtt_min,
+        present), each with min(k, live) rows.  Ties: ascending slot hash, then ascending key bytes."""
+        from ._lib import FA_TOP_BYTES, FA_TOP_PACKETS, EvictOut
+        metric = {"bytes": FA_TOP_BYTES, "packets": FA_TOP_PACKETS}[by]
+        rows = max(int(k), 1)
+        out, dns, add = np.zeros((rows, REC_BYTES), np.uint8), np.zeros((rows, 64), np.uint8), np.zeros((rows, 32), np.uint8)
+        drops, rmin, pres = np.zeros((rows, 32), np.uint8), np.zeros(rows, np.uint64), np.zeros(rows, np.uint8)
+        o = EvictOut(records=out.ctypes.data, dns=dns.ctypes.data, additional=add.ctypes.data, pkt_drops=drops.ctypes.data,
+                     rtt_min=rmin.ctypes.data, present=pres.ctypes.data)
+        got = C.c_size_t(0)
+        check(lib().fa_top_flows(self._h, metric, int(k), C.byref(o), C.byref(got)))
+        g = got.value
+        return out[:g], dns[:g], add[:g], drops[:g], rmin[:g], pres[:g]
+
     def read_spilled(self, cap=131072):
         """KERNEL_MAP mode with FA_F_RINGBUF_FALLBACK: the single-packet records that could not enter the full map
         (the batched equivalent of reading the direct_flows ring buffer) -> (n,144) uint8 array."""
