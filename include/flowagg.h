@@ -406,6 +406,26 @@ int fa_evict_ex(fa_engine* e, const fa_evict_out* out, size_t cap, size_t* n_out
 #define FA_TOP_MAX_K    (1u << 20)
 int fa_top_flows(fa_engine* e, uint32_t by, size_t k, const fa_evict_out* out, size_t* n_out);
 
+/* Point lookups of the flows the caller names (bpf_map_lookup_elem for a batch of keys), on the device, WITHOUT
+ * removing or changing anything (table, feature lines, counters, live flow count, sketch and DNS correlation table are
+ * as before; a later eviction returns what it would have returned without the call; fa_stats changes only in
+ * kernel_launches, h2d_bytes and d2h_bytes).
+ *   keys:   n x 40-byte fa_flow_id, host (pageable or pinned) or device memory; device keys 8-byte aligned.  Byte 39
+ *           (padding) is ignored, as on ingest.
+ *   Output: the blocks of `out` as in fa_evict_ex (`records` required, others may be NULL), each in host or device memory
+ *           on its own, each with room for n rows.  Row i is keys[i]: when its flow is live, row i of every block is
+ *           bit-identical to the row fa_evict_ex would return for that flow now (feature blocks, rtt_min, present and the
+ *           base patch of feature-only flows included); otherwise row i of every requested block is all zero.  A
+ *           requested block the engine does not produce comes back zero.  Duplicate keys each get their own row.
+ *   found:  n bytes (host or device; may be NULL): 1 if keys[i] is live, else 0.  *n_found = the number of found keys.
+ *   Runs on the engine stream after every queued fold, under the engine lock, and returns when the outputs are
+ *   complete.  Any n: the keys go through in chunks, device scratch and staging are O(chunk), allocated on first use.
+ *   Not looked up: with FA_F_NONBLOCKING_EVICT a retired table still being evicted (once fa_evict returns, every key it
+ *   evicted misses); the fallback ring (fa_read_spilled); DNS queries waiting for their response.
+ *   n == 0: FA_OK with *n_found = 0.  FA_E_INVAL: null engine / out / out->records / n_found, null keys with n > 0,
+ *   device keys not 8-byte aligned (nothing is written). */
+int fa_lookup_flows(fa_engine* e, const void* keys, size_t n, const fa_evict_out* out, uint8_t* found, size_t* n_found);
+
 /* Lookup-and-RESET (no reference analogue; building block of the multi-GPU local combiner, the counterpart of
  * the reference folding its per-CPU maps in user space, pkg/tracer/tracer.go:1159-1187): every flow that received
  * records since the previous drain is written to out_records (device memory, cap x 144 B) as a partial flow record

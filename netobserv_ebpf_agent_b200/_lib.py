@@ -80,6 +80,8 @@ SIGNATURES = {
     "fa_ingest_pkt_drops": (C.c_int, [C.c_void_p, C.c_void_p, C.c_size_t]),
     "fa_evict_ex": (C.c_int, [C.c_void_p, C.POINTER(EvictOut), C.c_size_t, C.POINTER(C.c_size_t)]),
     "fa_top_flows": (C.c_int, [C.c_void_p, C.c_uint32, C.c_size_t, C.POINTER(EvictOut), C.POINTER(C.c_size_t)]),
+    "fa_lookup_flows": (C.c_int, [C.c_void_p, C.c_void_p, C.c_size_t, C.POINTER(EvictOut), C.c_void_p,
+                                  C.POINTER(C.c_size_t)]),
     "fa_evict": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_size_t,
                            C.POINTER(C.c_size_t)]),
     "fa_drain_active": (C.c_int, [C.c_void_p, C.c_void_p, C.c_size_t, C.POINTER(C.c_size_t)]),

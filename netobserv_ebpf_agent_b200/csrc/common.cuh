@@ -215,4 +215,27 @@ __device__ __forceinline__ void red_min_u32(void* p, uint32_t v) { asm volatile(
 __device__ __forceinline__ uint64_t u64_of(uint32_t lo, uint32_t hi) { return (uint64_t)lo | ((uint64_t)hi << 32); }
 #endif  // __CUDACC__
 
+// ------------------------------------------------------------------ read-only table probe
+constexpr uint32_t kNoSlot = 0xFFFFFFFFu;   // a key without a live flow
+#if defined(__CUDACC__) || defined(FA_HOST_EMUL)
+// The slot of the key whose first three 16-byte chunks are k0, k1, k2 (slot hash h; the tag half of k2 and key byte 39
+// are ignored), or kNoSlot.  Linear probing from the home slot, one round trip per slot for the three line chunks that
+// hold the key and the tag (the tag shares a chunk with the key tail).  An EMPTY tag ends the walk (a miss), an equal
+// key is a hit; feature-only entries (published without TAG_HAS_BASE) are live flows and are found.  The walk visits
+// each slot at most once, so it also ends on a physically full table (FA_F_NO_FULL_CUT).  For a table no launch is
+// writing: the "full" cut pre-pass and fa_lookup_flows.
+__device__ __forceinline__ uint32_t table_find(const Table& t, uint64_t h, uint4 k0, uint4 k1, uint4 k2) {
+    uint64_t slot = h & t.mask;
+    for (uint64_t probes = 0; probes <= t.mask; probes++) {
+        const uint4* L = &t.ident[slot * 8];
+        const uint4 l0 = ld_cg_u4(L), l1 = ld_cg_u4(L + 1), l2 = ld_cg_u4(L + 2);
+        if ((l2.z & TAG_STATE_MASK) == 0) break;
+        if (eq4_masked(l0, k0, chunk_mask(0)) && eq4_masked(l1, k1, chunk_mask(1)) && eq4_masked(l2, k2, chunk_mask(2)))
+            return (uint32_t)slot;
+        slot = (slot + 1) & t.mask;
+    }
+    return kNoSlot;
+}
+#endif
+
 }  // namespace fa

@@ -152,6 +152,11 @@ struct fa_engine {
     Staging top_stage;                        // fa_top_flows: under `mu`
     fa::TopScratch top{};                     // fa_top_flows select state, histograms and candidates (cap entries)
     fa::TopState* h_top_state = nullptr;      // pinned
+    Staging lookup_stage;                     // fa_lookup_flows: under `mu`
+    uint32_t* d_lookup_slot = nullptr;        // fa_lookup_flows scratch of one chunk: each key's slot (or kNoSlot) ...
+    uint8_t* d_lookup_found = nullptr;        // ... and found flag (for a host `found`); lookup_cap keys
+    uint64_t lookup_cap = 0;
+    unsigned long long* d_lookup_hits = nullptr; unsigned long long* h_lookup_hits = nullptr;   // hit count; pinned mirror
     uint32_t* d_slot_of = nullptr;            // per-sample slot scratch of the feature folds
     uint64_t feat_seq[3] = {0, 0, 0};         // running sample numbers (additional, dns, packet drops)
     uint32_t* d_route_tmp = nullptr; unsigned long long* d_route_counts = nullptr;
@@ -675,6 +680,8 @@ void fa_destroy(fa_engine* e) {
     cudaFree(e->d_snap_src); cudaFree(e->d_snap_cnt); cudaFree(e->d_snap_verdict);
     free_staging(&e->evict_stage); free_staging(&e->top_stage); cudaFree(e->d_slot_of);
     cudaFree(e->top.state); cudaFree(e->top.hist); cudaFree(e->top.ents); if (e->h_top_state) cudaFreeHost(e->h_top_state);
+    free_staging(&e->lookup_stage); cudaFree(e->d_lookup_slot); cudaFree(e->d_lookup_found); cudaFree(e->d_lookup_hits);
+    if (e->h_lookup_hits) cudaFreeHost(e->h_lookup_hits);
     cudaFree(e->sk.cms); cudaFree(e->sk.hll);
     cudaFree(e->dnsc.tab); cudaFree(e->dnsc_spare); cudaFree(e->dnsc.ctr); cudaFreeHost(e->h_dnsc_ctr);
     cudaFree(e->d_dnsc_state); cudaFree(e->d_dnsc_samples); cudaFree(e->d_dnsc_out); cudaFree(e->d_dnsc_warps);
@@ -1092,6 +1099,71 @@ int fa_top_flows(fa_engine* e, uint32_t by, size_t k, const fa_evict_out* o, siz
     e->st.kernel_launches += launched;
     e->st.d2h_bytes += d2h;
     *n_out = (size_t)n;
+    return FA_OK;
+}
+
+// Exact point lookups of live flows by key, read in place (evict.cu: launch_lookup_flows).  Chunk by chunk on the engine
+// stream after the queued folds: the keys reach the device through Input, the probe writes each key's slot (or kNoSlot)
+// and counts the hits on the device, the gather and the feature pass (clear = false) fill the chunk's rows of every
+// block.  Device scratch and staging hold one chunk; one wait at the end.  Nothing of the table or the counters is written.
+int fa_lookup_flows(fa_engine* e, const void* keys, size_t n, const fa_evict_out* o, uint8_t* found, size_t* n_found) {
+    if (!e || !o || !o->records || !n_found || (!keys && n)) return fail(FA_E_INVAL, "fa_lookup_flows: null argument");
+    std::lock_guard<std::mutex> lk(e->mu);
+    CU(cudaSetDevice(e->device));
+    const uint64_t chunk = stage_records(e);
+    Input in(e, keys, n, fa::kKeyBytes, chunk, chunk, WINDOW_NONE);
+    if (n && in.misaligned(8)) return fail(FA_E_INVAL, "fa_lookup_flows: device keys must be 8-byte aligned");
+    *n_found = 0;
+    if (n == 0) return FA_OK;
+    const fa::Table t = e->table;
+    const bool kmap = e->cfg.mode == FA_MODE_KERNEL_MAP;
+    const bool feats = t.feat_add || t.feat_dns || t.feat_drop;
+    const bool found_dev = found && classify(found) == PTR_DEVICE;
+    cudaStream_t st = e->stream;
+    const uint64_t rows = std::min<uint64_t>(n, chunk);
+    if (int rc = grow_staging(e, &e->lookup_stage, rows, classify(o->records) != PTR_DEVICE, feats)) return rc;
+    if (e->lookup_cap < rows) {
+        cudaFree(e->d_lookup_slot); cudaFree(e->d_lookup_found);
+        e->d_lookup_slot = nullptr; e->d_lookup_found = nullptr; e->lookup_cap = 0;
+        CU(cudaMalloc(&e->d_lookup_slot, rows * 4)); CU(cudaMalloc(&e->d_lookup_found, rows));
+        e->lookup_cap = rows;
+    }
+    if (!e->d_lookup_hits) {
+        CU(cudaMalloc(&e->d_lookup_hits, 8));
+        CU(cudaHostAlloc(&e->h_lookup_hits, 8, cudaHostAllocDefault));
+    }
+    CU(cudaMemsetAsync(e->d_lookup_hits, 0, 8, st));
+    uint64_t launched = 0, d2h = 0;
+    while (in.more()) {
+        const uint8_t* d_keys = nullptr;
+        uint64_t c = 0;
+        if (int rc = in.next(&d_keys, &c)) return rc;
+        const size_t at = in.done;
+        auto row = [at](void* p, size_t width) { return p ? static_cast<uint8_t*>(p) + at * width : nullptr; };
+        fa_evict_out oc{};                             // the chunk's rows of every block
+        oc.records = row(o->records, fa::kRecBytes); oc.dns = row(o->dns, 64); oc.additional = row(o->additional, 32);
+        oc.pkt_drops = row(o->pkt_drops, 32); oc.rtt_min = reinterpret_cast<uint64_t*>(row(o->rtt_min, 8));
+        oc.present = row(o->present, 1);
+        Blocks d;
+        if (int rc = place_blocks(t, &oc, c, e->lookup_stage, st, &d)) return rc;
+        d.slot_of = e->d_lookup_slot;                  // the feature pass reads the probe's slots (kNoSlot: zero rows)
+        uint8_t* d_found = found_dev ? found + at : found ? e->d_lookup_found : nullptr;
+        launched += fa::launch_lookup_flows(t, kmap, reinterpret_cast<const uint64_t*>(d_keys), c, e->d_lookup_slot, d_found,
+                                            e->d_lookup_hits, d.rec, e->sm_count, st);
+        if (int rc = in.release()) return rc;
+        if (int rc = finish_blocks(e, t, &oc, c, d, /*clear=*/false, st, &launched, &d2h)) return rc;
+        if (found && !found_dev) {
+            CU(cudaMemcpyAsync(found + at, d_found, c, cudaMemcpyDeviceToHost, st));
+            d2h += c;
+        }
+        in.advance(c);
+    }
+    CU(cudaMemcpyAsync(e->h_lookup_hits, e->d_lookup_hits, 8, cudaMemcpyDeviceToHost, st));
+    CU(cudaStreamSynchronize(st));
+    if (int rc = in.finish(FA_OK, nullptr)) return rc;
+    e->st.kernel_launches += launched;
+    e->st.d2h_bytes += d2h;
+    *n_found = (size_t)*e->h_lookup_hits;
     return FA_OK;
 }
 

@@ -321,29 +321,38 @@ __global__ void __launch_bounds__(256) top_merge_kernel(Table t, TopEnt* e, unsi
     }
 }
 
-// the first n sorted entries as records, ACCOUNTER layout (emit_record, 4 flows per warp step) ...
-__global__ void __launch_bounds__(256) top_gather_kernel(Table t, const TopEnt* __restrict__ e, unsigned long long n,
-                                                         uint4* __restrict__ out, uint32_t* __restrict__ slot_of_out) {
+// Row i of `out` from the flow at slots[i * stride]: the sorted fa_top_flows candidates (stride: one TopEnt) or the
+// fa_lookup_flows probe results (stride 1).  kNoSlot: no flow; the row is written all zero when zero_miss (a lookup
+// miss), else left unwritten (padding in the first n of top-k: fewer candidates than n, the host reports it).
+// slot_of_out (optional, for the feature pass): the row's slot, 0 without a flow (read only by the peek).
+// ACCOUNTER layout (emit_record, 4 flows per warp step) ...
+__global__ void __launch_bounds__(256) gather_kernel(Table t, const uint32_t* __restrict__ slots, uint32_t stride, unsigned long long n,
+                                                     bool zero_miss, uint4* __restrict__ out, uint32_t* __restrict__ slot_of_out) {
     const int lane = threadIdx.x & 31, g = lane >> 3, j = lane & 7;
     const unsigned long long warp_global = (blockIdx.x * (unsigned long long)blockDim.x + threadIdx.x) >> 5;
     const unsigned long long n_warps = ((unsigned long long)gridDim.x * blockDim.x) >> 5;
     for (unsigned long long f0 = warp_global * 4; f0 < n; f0 += n_warps * 4) {
         const unsigned long long i = f0 + g;
-        const uint32_t s = i < n ? e[i].slot : kTopNoSlot;
-        const bool live = s != kTopNoSlot;                // padding in the first n: fewer candidates than n (the host
-        const uint64_t slot = live ? s : 0u;               // reports it); the row is left unwritten
-        emit_record(t, slot, live, live, out + i * kRecChunks, g, j);
-        if (slot_of_out && i < n && j == 0) slot_of_out[i] = (uint32_t)slot;   // padding: slot 0, read only by the peek
+        const uint32_t s = i < n ? slots[i * stride] : kNoSlot;
+        const bool live = s != kNoSlot;
+        const uint64_t slot = live ? s : 0u;
+        emit_record(t, slot, live, live || (zero_miss && i < n), out + i * kRecChunks, g, j);   // live = false: zeros
+        if (slot_of_out && i < n && j == 0) slot_of_out[i] = (uint32_t)slot;
     }
 }
 // ... and KERNEL_MAP layout (km_emit_record)
-__global__ void __launch_bounds__(256) top_gather_kmap_kernel(Table t, const TopEnt* __restrict__ e, unsigned long long n,
-                                                              uint8_t* __restrict__ out, uint32_t* __restrict__ slot_of_out) {
+__global__ void __launch_bounds__(256) gather_kmap_kernel(Table t, const uint32_t* __restrict__ slots, uint32_t stride,
+                                                          unsigned long long n, bool zero_miss, uint8_t* __restrict__ out,
+                                                          uint32_t* __restrict__ slot_of_out) {
     for (unsigned long long i = blockIdx.x * (unsigned long long)blockDim.x + threadIdx.x; i < n; i += (unsigned long long)gridDim.x * blockDim.x) {
-        const uint32_t slot = e[i].slot;
-        if (slot_of_out) slot_of_out[i] = slot == kTopNoSlot ? 0u : slot;   // padding: slot 0, read only by the peek
-        if (slot == kTopNoSlot) continue;                 // padding: fewer candidates than n (the host reports it)
-        km_emit_record(t, t.met, slot, out + i * kRecBytes);
+        const uint32_t slot = slots[i * stride];
+        if (slot_of_out) slot_of_out[i] = slot == kNoSlot ? 0u : slot;
+        if (slot != kNoSlot) {
+            km_emit_record(t, t.met, slot, out + i * kRecBytes);
+        } else if (zero_miss) {
+            uint64_t* O = reinterpret_cast<uint64_t*>(out + i * kRecBytes);
+            for (int k = 0; k < kRecBytes / 8; k++) O[k] = 0ull;
+        }
     }
 }
 
@@ -379,9 +388,51 @@ int launch_top_flows(const Table& t, bool kmap, const TopMetric& M, uint64_t n, 
         FA_LAUNCH(top_sort_tile_kernel, tiles, kTopSortTile / 2, tile_smem, st, t, s.ents, s.state, s.cap, size);
         launches++;
     }
-    if (kmap) FA_LAUNCH(top_gather_kmap_kernel, grid, 256, 0, st, t, s.ents, n, out_recs, slot_of_out);
-    else FA_LAUNCH(top_gather_kernel, grid, 256, 0, st, t, s.ents, n, reinterpret_cast<uint4*>(out_recs), slot_of_out);
+    const uint32_t* ent_slots = reinterpret_cast<const uint32_t*>(reinterpret_cast<const uint8_t*>(s.ents) + offsetof(TopEnt, slot));
+    const uint32_t ent_stride = sizeof(TopEnt) / sizeof(uint32_t);
+    if (kmap) FA_LAUNCH(gather_kmap_kernel, grid, 256, 0, st, t, ent_slots, ent_stride, n, false, out_recs, slot_of_out);
+    else FA_LAUNCH(gather_kernel, grid, 256, 0, st, t, ent_slots, ent_stride, n, false, reinterpret_cast<uint4*>(out_recs), slot_of_out);
     return launches + 1;
+}
+
+// ---- fa_lookup_flows: exact point lookups of live flows by key, without removing or changing anything -------------
+// One thread per key: table_find from the key's home slot, its slot (or kNoSlot) into slots[i] and found[i] (optional),
+// one hit-count atomic per warp step.  Keys are 40-byte fa_flow_id rows, read as five 8-byte words.
+__global__ void __launch_bounds__(256) lookup_probe_kernel(Table t, const uint64_t* __restrict__ keys, unsigned long long n,
+                                                           uint32_t* __restrict__ slots, uint8_t* __restrict__ found,
+                                                           unsigned long long* __restrict__ hits) {
+    const int lane = threadIdx.x & 31;
+    // warp-uniform steps (n is not a multiple of 32): every lane reaches the ballot
+    for (unsigned long long i0 = blockIdx.x * (unsigned long long)blockDim.x + (threadIdx.x & ~31u); i0 < n;
+         i0 += (unsigned long long)gridDim.x * blockDim.x) {
+        const unsigned long long i = i0 + lane;
+        uint32_t slot = kNoSlot;
+        if (i < n) {
+            const uint64_t* K = keys + i * (kKeyBytes / 8);
+            const uint64_t w0 = K[0], w1 = K[1], w2 = K[2], w3 = K[3], w4 = K[4];
+            const uint4 k0 = make_uint4((uint32_t)w0, (uint32_t)(w0 >> 32), (uint32_t)w1, (uint32_t)(w1 >> 32));
+            const uint4 k1 = make_uint4((uint32_t)w2, (uint32_t)(w2 >> 32), (uint32_t)w3, (uint32_t)(w3 >> 32));
+            const uint4 k2 = make_uint4((uint32_t)w4, (uint32_t)(w4 >> 32), 0u, 0u);
+            slot = table_find(t, slot_hash(key_premix(w0, w1, w2, w3, w4)), k0, k1, k2);
+            slots[i] = slot;
+            if (found) found[i] = slot != kNoSlot ? 1 : 0;
+        }
+        const uint32_t hit = __ballot_sync(0xFFFFFFFFu, slot != kNoSlot);
+        if (lane == 0 && hit) atomicAdd(hits, (unsigned long long)__popc(hit));
+    }
+}
+
+// One text for the device and the host emulation (FA_LAUNCH): the probe, then the gather of the rows (zero for misses).
+int launch_lookup_flows(const Table& t, bool kmap, const uint64_t* keys, uint64_t n, uint32_t* slots, uint8_t* found,
+                        unsigned long long* hits, uint8_t* out_recs, int sm_count, cudaStream_t st) {
+    if (!n) return 0;
+    const uint64_t cap = (uint64_t)sm_count * 8;
+    const uint64_t per_key = (n + 255) / 256, per_lanes = (n * 8 + 255) / 256;      // a thread per key / 8 lanes per row
+    const int g_probe = (int)(per_key < cap ? per_key : cap), g_rows = (int)(per_lanes < cap ? per_lanes : cap);
+    FA_LAUNCH(lookup_probe_kernel, g_probe, 256, 0, st, t, keys, n, slots, found, hits);
+    if (kmap) FA_LAUNCH(gather_kmap_kernel, g_probe, 256, 0, st, t, slots, 1u, n, true, out_recs, nullptr);
+    else FA_LAUNCH(gather_kernel, g_rows, 256, 0, st, t, slots, 1u, n, true, reinterpret_cast<uint4*>(out_recs), nullptr);
+    return 2;
 }
 
 }  // namespace fa

@@ -406,7 +406,8 @@ __device__ __forceinline__ void build_base(uint64_t& bs, uint64_t& be, uint32_t&
     if (beth == 0 && neth != 0) beth = (uint32_t)(~neth) & 0xFFFFu;
 }
 
-// kClear = false: the fa_top_flows peek, which emits the same rows and leaves the feature lines as they are.
+// kClear = false: the fa_top_flows / fa_lookup_flows peek, which emits the same rows and leaves the feature lines as
+// they are; a row whose slot is kNoSlot (a lookup miss) gets zero feature rows and present = 0.
 template <bool kClear = true>
 __global__ void evict_features_kernel(Table t, const uint32_t* __restrict__ slot_of_out, unsigned long long n_out,
                                       uint8_t* __restrict__ out_recs, uint8_t* __restrict__ out_dns,
@@ -415,6 +416,14 @@ __global__ void evict_features_kernel(Table t, const uint32_t* __restrict__ slot
     for (unsigned long long i = blockIdx.x * (unsigned long long)blockDim.x + threadIdx.x; i < n_out;
          i += (unsigned long long)gridDim.x * blockDim.x) {
         const uint32_t slot = slot_of_out[i];
+        if (!kClear && slot == kNoSlot) {
+            if (t.feat_dns && out_dns) for (int c = 0; c < 8; c++) reinterpret_cast<uint64_t*>(out_dns + i * 64)[c] = 0ull;
+            if (t.feat_drop && out_drop) for (int c = 0; c < 4; c++) reinterpret_cast<uint64_t*>(out_drop + i * 32)[c] = 0ull;
+            if (t.feat_add && out_add) for (int c = 0; c < 4; c++) reinterpret_cast<uint64_t*>(out_add + i * 32)[c] = 0ull;
+            if (out_rtt_min) out_rtt_min[i] = 0ull;
+            if (out_present) out_present[i] = 0;
+            continue;
+        }
         uint8_t* O = out_recs + i * kRecBytes;
         uint64_t bs = *reinterpret_cast<uint64_t*>(O + R_START), be = *reinterpret_cast<uint64_t*>(O + R_END);
         uint32_t beth = *reinterpret_cast<uint16_t*>(O + R_ETH);

@@ -65,7 +65,7 @@ int launch_feature_fold(int kind, const uint8_t* recs, uint32_t n, const Table& 
 int launch_evict_features(const Table& t, const uint32_t* slot_of_out, unsigned long long n_out, uint8_t* out_recs,
                           uint8_t* out_dns, uint8_t* out_add, uint8_t* out_drop, unsigned long long* out_rtt_min,
                           uint8_t* out_present, int sm_count, cudaStream_t st);
-// the same rows for fa_top_flows, leaving the feature lines as they are
+// the same rows for fa_top_flows / fa_lookup_flows, leaving the feature lines as they are (slot kNoSlot: zero rows)
 int launch_peek_features(const Table& t, const uint32_t* slot_of_out, unsigned long long n_out, uint8_t* out_recs,
                          uint8_t* out_dns, uint8_t* out_add, uint8_t* out_drop, unsigned long long* out_rtt_min,
                          uint8_t* out_present, int sm_count, cudaStream_t st);
@@ -75,7 +75,7 @@ int launch_peek_features(const Table& t, const uint32_t* slot_of_out, unsigned l
 struct TopMetric { const uint8_t* p; uint32_t stride; uint32_t wide; };
 // one compacted candidate; slot == kTopNoSlot marks the padding that sorts last
 struct TopEnt { unsigned long long m, h; uint32_t slot, pad; };
-constexpr uint32_t kTopNoSlot = 0xFFFFFFFFu;
+constexpr uint32_t kTopNoSlot = kNoSlot;
 constexpr int kTopPasses = 16;                     // 8-bit digits of the 128-bit composite; later passes exit at once
 constexpr int kTopSortTile = 1024;                 // entries sorted in shared memory by one CTA
 constexpr uint64_t kTopSlack = 4096;               // compaction room beyond k: the select stops once the candidates fit
@@ -102,6 +102,12 @@ struct TopScratch {
 // slot_of_out (optional, for the feature pass).  kmap: KERNEL_MAP record layout.  Nothing in `t` changes.
 int launch_top_flows(const Table& t, bool kmap, const TopMetric& M, uint64_t n, uint64_t live, const TopScratch& s,
                      uint8_t* out_recs, uint32_t* slot_of_out, int sm_count, cudaStream_t st);
+
+// fa_lookup_flows (evict.cu): for each of the n 40-byte keys (device, 8-byte aligned) its slot in `t` or kNoSlot into
+// slots (the feature pass reads them), 1 / 0 into found (optional), the number of hits added to *hits, and its row into
+// out_recs (device, n x 144 B; all zero without a flow).  kmap: KERNEL_MAP record layout.  Nothing in `t` changes.
+int launch_lookup_flows(const Table& t, bool kmap, const uint64_t* keys, uint64_t n, uint32_t* slots, uint8_t* found,
+                        unsigned long long* hits, uint8_t* out_recs, int sm_count, cudaStream_t st);
 
 // sketches
 int launch_cms_query(const SketchParams& sk, const uint4* keys, uint32_t n, unsigned long long* est, cudaStream_t st);

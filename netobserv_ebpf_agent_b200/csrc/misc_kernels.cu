@@ -69,18 +69,7 @@ __global__ void cut_scan_kernel(const uint4* __restrict__ recs, uint32_t n, Tabl
         const uint4 k0 = R[0], k1 = R[1], k2 = R[2];
         const uint64_t h = slot_hash(key_premix(u64_of(k0.x, k0.y), u64_of(k0.z, k0.w), u64_of(k1.x, k1.y),
                                                 u64_of(k1.z, k1.w), u64_of(k2.x, k2.y)));
-        uint64_t slot = h & t.mask;
-        bool exists = false;
-        for (;;) {
-            const unsigned long long tag = ld_cg_u64(reinterpret_cast<const unsigned long long*>(&t.ident[slot * 8 + 2]) + 1);
-            if ((tag & TAG_STATE_MASK) == 0) break;
-            const uint4 l0 = ld_cg_u4(&t.ident[slot * 8]), l1 = ld_cg_u4(&t.ident[slot * 8 + 1]), l2 = ld_cg_u4(&t.ident[slot * 8 + 2]);
-            if (eq4_masked(l0, k0, chunk_mask(0)) && eq4_masked(l1, k1, chunk_mask(1)) && eq4_masked(l2, k2, chunk_mask(2))) {
-                exists = true; break;
-            }
-            slot = (slot + 1) & t.mask;
-        }
-        if (exists) continue;
+        if (table_find(t, h, k0, k1, k2) != kNoSlot) continue;     // the flow exists
         uint32_t s = (uint32_t)(h >> 24) & set_mask;
         for (;;) {
             uint32_t cur = atomicCAS(&idx_set[s], kSetEmpty, i);

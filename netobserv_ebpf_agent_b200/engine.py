@@ -183,6 +183,23 @@ class FlowAggEngine:
         g = got.value
         return out[:g], dns[:g], add[:g], drops[:g], rmin[:g], pres[:g]
 
+    def lookup_flows(self, keys):
+        """Exact point lookups of live flows, without removing or changing anything: keys, (m, 40) uint8 flow ids in
+        host memory -> the six arrays of evict_ex (records, dns, additional, pkt_drops, rtt_min, present) and found
+        (m,) uint8, each with m rows.  Row i is keys[i]; its rows are all zero where found[i] == 0."""
+        from ._lib import ID_BYTES, EvictOut
+        k = np.ascontiguousarray(keys, dtype=np.uint8).reshape(-1, ID_BYTES)
+        m = len(k)
+        rows = max(m, 1)
+        out, dns, add = np.zeros((rows, REC_BYTES), np.uint8), np.zeros((rows, 64), np.uint8), np.zeros((rows, 32), np.uint8)
+        drops, rmin, pres = np.zeros((rows, 32), np.uint8), np.zeros(rows, np.uint64), np.zeros(rows, np.uint8)
+        found = np.zeros(rows, np.uint8)
+        o = EvictOut(records=out.ctypes.data, dns=dns.ctypes.data, additional=add.ctypes.data, pkt_drops=drops.ctypes.data,
+                     rtt_min=rmin.ctypes.data, present=pres.ctypes.data)
+        got = C.c_size_t(0)
+        check(lib().fa_lookup_flows(self._h, k.ctypes.data, m, C.byref(o), found.ctypes.data, C.byref(got)))
+        return out[:m], dns[:m], add[:m], drops[:m], rmin[:m], pres[:m], found[:m]
+
     def read_spilled(self, cap=131072):
         """KERNEL_MAP mode with FA_F_RINGBUF_FALLBACK: the single-packet records that could not enter the full map
         (the batched equivalent of reading the direct_flows ring buffer) -> (n,144) uint8 array."""
