@@ -19,7 +19,7 @@
  * caller is expected to handle (FA_FULL).
  *
  * Threading: at most one thread in fa_ingest*() and one other thread in
- * fa_evict()/fa_purge_stale_dns() at the same time (exactly the reference's
+ * fa_evict()/fa_expire_flows()/fa_purge_stale_dns() at the same time (the reference's
  * model: one RingBufTracer/Accounter goroutine, one single-flight evictor —
  * pkg/flow/tracer_map.go:83-101).  The engine never retains a host pointer
  * after the call that received it returns.
@@ -425,6 +425,32 @@ int fa_top_flows(fa_engine* e, uint32_t by, size_t k, const fa_evict_out* out, s
  *   n == 0: FA_OK with *n_found = 0.  FA_E_INVAL: null engine / out / out->records / n_found, null keys with n > 0,
  *   device keys not 8-byte aligned (nothing is written). */
 int fa_lookup_flows(fa_engine* e, const void* keys, size_t n, const fa_evict_out* out, uint8_t* found, size_t* n_found);
+
+/* Flow expiry on the two timers of NetFlow / IPFIX exporters, OVS and conntrack: lookup-and-delete only the live flows
+ * past an idle or an active timeout, on the device; every other flow stays live (no reference analogue: the reference
+ * evicts the whole window every CACHE_ACTIVE_TIMEOUT).
+ *   Expires: a live flow with (idle_timeout_ns != 0 and (int64_t)(mono_now_ns - end) >= (int64_t)idle_timeout_ns) or
+ *            (active_timeout_ns != 0 and (int64_t)(mono_now_ns - start) >= (int64_t)active_timeout_ns), where start and
+ *            end are start_mono_time_ts / end_mono_time_ts (record offsets 40 / 48) of the row fa_evict_ex would return
+ *            for it now (base patch of feature-only flows and feature effects included).  The compare is signed, as in
+ *            fa_purge_stale_dns: a zero timestamp is infinitely old, a timestamp after mono_now_ns (skewed per-CPU
+ *            clocks) never expires.
+ *   Output: the blocks of `out` as in fa_evict_ex (`records` required, others may be NULL; host or device memory), each
+ *           with room for cap rows: the expired flows' rows, bit-identical to fa_evict_ex's (feature blocks, rtt_min,
+ *           present and base patch included), in unspecified order.  A requested block the engine does not produce comes
+ *           back zero.  *n_out = the number of expired flows.  They are removed with their metric and feature lines; every
+ *           other flow keeps every field bit for bit (its slot may move), and later folds into it go on as before.
+ *   Stats:  flows_evicted += *n_out, evictions += 1, live_flows -= *n_out, kernel_launches and d2h_bytes as usual; the
+ *           sketch, the DNS correlation table and the fallback ring are untouched.
+ *   Runs on the engine stream after every queued fold, under the engine lock (the evictor side of the threading
+ *   contract; fa_ingest* waits for it as for a blocking eviction), and returns when the outputs are complete.  Both
+ *   modes; FA_F_NONBLOCKING_EVICT: expires the live table only.  ACCOUNTER mode after FA_FULL: expire instead of
+ *   evicting, then resume fa_ingest at *consumed; the next cut is computed against the new live count.  Device scratch:
+ *   slots / 8 bytes + 4 bytes per live flow, allocated on first use.
+ *   FA_E_2BIG: more than cap flows would expire; *n_out = that count and nothing changes.
+ *   FA_E_INVAL: null engine / out / out->records / n_out, both timeouts zero, a timeout above INT64_MAX (nothing changes). */
+int fa_expire_flows(fa_engine* e, uint64_t mono_now_ns, uint64_t idle_timeout_ns, uint64_t active_timeout_ns,
+                    const fa_evict_out* out, size_t cap, size_t* n_out);
 
 /* Lookup-and-RESET (no reference analogue; building block of the multi-GPU local combiner, the counterpart of
  * the reference folding its per-CPU maps in user space, pkg/tracer/tracer.go:1159-1187): every flow that received

@@ -82,6 +82,8 @@ SIGNATURES = {
     "fa_top_flows": (C.c_int, [C.c_void_p, C.c_uint32, C.c_size_t, C.POINTER(EvictOut), C.POINTER(C.c_size_t)]),
     "fa_lookup_flows": (C.c_int, [C.c_void_p, C.c_void_p, C.c_size_t, C.POINTER(EvictOut), C.c_void_p,
                                   C.POINTER(C.c_size_t)]),
+    "fa_expire_flows": (C.c_int, [C.c_void_p, C.c_uint64, C.c_uint64, C.c_uint64, C.POINTER(EvictOut), C.c_size_t,
+                                  C.POINTER(C.c_size_t)]),
     "fa_evict": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_size_t,
                            C.POINTER(C.c_size_t)]),
     "fa_drain_active": (C.c_int, [C.c_void_p, C.c_void_p, C.c_size_t, C.POINTER(C.c_size_t)]),

@@ -157,6 +157,9 @@ struct fa_engine {
     uint8_t* d_lookup_found = nullptr;        // ... and found flag (for a host `found`); lookup_cap keys
     uint64_t lookup_cap = 0;
     unsigned long long* d_lookup_hits = nullptr; unsigned long long* h_lookup_hits = nullptr;   // hit count; pinned mirror
+    Staging expire_stage;                     // fa_expire_flows: under `mu`
+    fa::ExpireScratch expire{};               // fa_expire_flows: expire bitmap, slot list (cap entries), counters
+    fa::ExpireCtr* h_expire_ctr = nullptr;    // pinned
     uint32_t* d_slot_of = nullptr;            // per-sample slot scratch of the feature folds
     uint64_t feat_seq[3] = {0, 0, 0};         // running sample numbers (additional, dns, packet drops)
     uint32_t* d_route_tmp = nullptr; unsigned long long* d_route_counts = nullptr;
@@ -682,6 +685,8 @@ void fa_destroy(fa_engine* e) {
     cudaFree(e->top.state); cudaFree(e->top.hist); cudaFree(e->top.ents); if (e->h_top_state) cudaFreeHost(e->h_top_state);
     free_staging(&e->lookup_stage); cudaFree(e->d_lookup_slot); cudaFree(e->d_lookup_found); cudaFree(e->d_lookup_hits);
     if (e->h_lookup_hits) cudaFreeHost(e->h_lookup_hits);
+    free_staging(&e->expire_stage); cudaFree(e->expire.bm); cudaFree(e->expire.list); cudaFree(e->expire.ctr);
+    if (e->h_expire_ctr) cudaFreeHost(e->h_expire_ctr);
     cudaFree(e->sk.cms); cudaFree(e->sk.hll);
     cudaFree(e->dnsc.tab); cudaFree(e->dnsc_spare); cudaFree(e->dnsc.ctr); cudaFreeHost(e->h_dnsc_ctr);
     cudaFree(e->d_dnsc_state); cudaFree(e->d_dnsc_samples); cudaFree(e->d_dnsc_out); cudaFree(e->d_dnsc_warps);
@@ -1164,6 +1169,70 @@ int fa_lookup_flows(fa_engine* e, const void* keys, size_t n, const fa_evict_out
     e->st.kernel_launches += launched;
     e->st.d2h_bytes += d2h;
     *n_found = (size_t)*e->h_lookup_hits;
+    return FA_OK;
+}
+
+// Remove only the live flows past an idle or active timeout (evict.cu: launch_expire_*), on the engine stream after the
+// queued folds: the mark writes the expire bitmap and slot list and counts them (one wait, to check cap), the gather and
+// the clearing feature pass emit their rows, then the delete pass removes them and compacts their clusters in place.
+// Every other flow stays live, bit for bit.  FA_F_NONBLOCKING_EVICT: the live table only; the spare stays empty.
+int fa_expire_flows(fa_engine* e, uint64_t mono_now_ns, uint64_t idle_timeout_ns, uint64_t active_timeout_ns,
+                    const fa_evict_out* o, size_t cap, size_t* n_out) {
+    if (n_out) *n_out = 0;
+    if (!e || !o || !o->records || !n_out) return fail(FA_E_INVAL, "fa_expire_flows: null argument");
+    if (!idle_timeout_ns && !active_timeout_ns) return fail(FA_E_INVAL, "fa_expire_flows: both timeouts are zero");
+    if (idle_timeout_ns > (uint64_t)INT64_MAX || active_timeout_ns > (uint64_t)INT64_MAX)
+        return fail(FA_E_INVAL, "fa_expire_flows: a timeout above INT64_MAX");
+    std::lock_guard<std::mutex> lk(e->mu);
+    CU(cudaSetDevice(e->device));
+    if (int rc = sync_counters(e)) return rc;          // the queued folds finish; exact live count
+    const uint64_t live = e->live_known;
+    if (live == 0) { e->st.evictions++; return FA_OK; }
+    const fa::Table t = e->table;
+    const bool kmap = e->cfg.mode == FA_MODE_KERNEL_MAP;
+    const bool feats = t.feat_add || t.feat_dns || t.feat_drop;
+    cudaStream_t st = e->stream;
+    if (!e->expire.bm) {
+        CU(cudaMalloc(&e->expire.bm, e->slots / 8));
+        CU(cudaMalloc(&e->expire.ctr, sizeof(fa::ExpireCtr)));
+        CU(cudaHostAlloc(&e->h_expire_ctr, sizeof(fa::ExpireCtr), cudaHostAllocDefault));
+    }
+    if (e->expire.cap < live) {                        // room for every live flow: the list never overflows
+        cudaFree(e->expire.list); e->expire.list = nullptr; e->expire.cap = 0;
+        const uint64_t want = std::max<uint64_t>(live, std::min<uint64_t>(e->slots, 2 * live));
+        CU(cudaMalloc(&e->expire.list, want * 4));
+        e->expire.cap = want;
+    }
+    const fa::ExpireScratch s = e->expire;
+    CU(cudaMemsetAsync(s.ctr, 0, sizeof(fa::ExpireCtr), st));
+    uint64_t launched = fa::launch_expire_mark(t, mono_now_ns, idle_timeout_ns, active_timeout_ns, s, e->sm_count, st);
+    CU(cudaGetLastError());
+    CU(cudaMemcpyAsync(e->h_expire_ctr, s.ctr, sizeof(fa::ExpireCtr), cudaMemcpyDeviceToHost, st));
+    CU(cudaStreamSynchronize(st));
+    const uint64_t n = e->h_expire_ctr->n;
+    if (n > live) return fail(FA_E_CUDA, "fa_expire_flows: the mark found %llu flows, counter says %llu live", (unsigned long long)n,
+                              (unsigned long long)live);
+    if (n > cap) {
+        *n_out = (size_t)n;
+        return fail(FA_E_2BIG, "fa_expire_flows: capacity %zu < %llu expiring flows", cap, (unsigned long long)n);
+    }
+    uint64_t d2h = 0;
+    if (n) {
+        if (int rc = grow_staging(e, &e->expire_stage, n, classify(o->records) != PTR_DEVICE, feats)) return rc;
+        Blocks d;
+        if (int rc = place_blocks(t, o, n, e->expire_stage, st, &d)) return rc;
+        launched += fa::launch_expire_emit(t, kmap, s, n, d.rec, d.slot_of, e->sm_count, st);
+        if (int rc = finish_blocks(e, t, o, n, d, /*clear=*/true, st, &launched, &d2h)) return rc;
+        launched += fa::launch_expire_delete(t, s, n, live == e->slots, e->d_ctr, e->sm_count, st);
+        CU(cudaGetLastError());
+        CU(cudaStreamSynchronize(st));
+        set_live_known(e, live - n);
+    }
+    e->st.evictions++;
+    e->st.flows_evicted += n;
+    e->st.kernel_launches += launched;
+    e->st.d2h_bytes += d2h;
+    *n_out = (size_t)n;
     return FA_OK;
 }
 

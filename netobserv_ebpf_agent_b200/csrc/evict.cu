@@ -435,4 +435,192 @@ int launch_lookup_flows(const Table& t, bool kmap, const uint64_t* keys, uint64_
     return 2;
 }
 
+// ---- fa_expire_flows: remove only the flows past an idle or active timeout, in place -------------------------------
+// Mark (bitmap-driven, like top_hist_kernel): each live flow's row start / end, patched by its feature lines as the
+// eviction patches them, against the two timeouts -> expire bitmap + slot list.  Emit: the gather of fa_lookup_flows
+// over the list, then the clearing feature pass.  Delete: a cluster is a maximal cyclic run of occupied slots; its
+// bounds were EMPTY before the call and stay EMPTY, so clusters are independent and one thread takes each cluster that
+// holds an expiring flow: it clears the expiring slots, then vacates each survivor in cluster order and re-inserts it
+// by linear probing from its home slot (never past its old position, so the walk never overwrites an entry it has not
+// reached).  Every key stays reachable from its home slot without crossing an EMPTY slot: K1, K6, the KERNEL_MAP
+// resolve and table_find find it as before.  A table without an EMPTY slot has no cluster bound: one thread runs
+// backward-shift deletion over it.
+
+__device__ __forceinline__ bool bit_at(const uint32_t* bm, uint64_t s) { return (bm[s >> 5] >> (s & 31)) & 1u; }
+__device__ __forceinline__ bool expire_due(uint64_t now, uint64_t ts, uint64_t timeout) {
+    return timeout != 0 && (int64_t)(now - ts) >= (int64_t)timeout;   // signed, as time.Duration: a zero ts is infinitely old
+}
+// The start / end of the row fa_evict_ex would return for `slot` now: the hot line (ACCOUNTER) or the metric line
+// (KERNEL_MAP), patched with the effects of its feature lines in the eviction's order (evict_features_kernel).
+__device__ __forceinline__ void row_times(const Table& t, uint64_t slot, uint64_t& bs, uint64_t& be) {
+    if (t.met) {
+        const uint8_t* M = t.met + slot * kMetLineBytes;
+        bs = km_ld64(M + KM_START); be = km_ld64(M + KM_END);
+    } else {
+        const uint64_t* H = reinterpret_cast<const uint64_t*>(t.hot + slot * 2);
+        bs = 0ull - H[1]; be = H[2];                               // nstart = 0 - start; 0 stays 0
+    }
+    uint32_t beth = 0;
+    if (t.feat_dns) { const uint64_t* S = reinterpret_cast<const uint64_t*>(t.feat_dns + slot * kDnsState); if (S[0]) build_base(bs, be, beth, S[4], S[5], 0); }
+    if (t.feat_drop) { const uint64_t* S = reinterpret_cast<const uint64_t*>(t.feat_drop + slot * kDropState); if (S[0]) build_base(bs, be, beth, S[6], S[7], 0); }
+    if (t.feat_add) { const uint64_t* S = reinterpret_cast<const uint64_t*>(t.feat_add + slot * kAddState); if (S[0]) build_base(bs, be, beth, S[3], S[4], 0); }
+}
+// Exclusive prefix of cnt over the warp and one cursor atomic for the warp's total: this lane's first index.  Every lane
+// of the warp calls it.
+__device__ __forceinline__ unsigned long long warp_reserve(uint32_t cnt, unsigned long long* cursor) {
+    const int lane = threadIdx.x & 31;
+    uint32_t incl = cnt;
+#pragma unroll
+    for (int d = 1; d < 32; d <<= 1) { const uint32_t v = __shfl_up_sync(0xFFFFFFFFu, incl, d); if (lane >= d) incl += v; }
+    const uint32_t total = __shfl_sync(0xFFFFFFFFu, incl, 31);
+    unsigned long long base = 0;
+    if (lane == 0 && total) base = atomicAdd(cursor, (unsigned long long)total);
+    base = __shfl_sync(0xFFFFFFFFu, base, 0);
+    return base + incl - cnt;
+}
+
+__global__ void __launch_bounds__(256) expire_mark_kernel(Table t, uint64_t now, uint64_t idle, uint64_t active, uint32_t* __restrict__ bm,
+                                                          uint32_t* __restrict__ list, unsigned long long cap, ExpireCtr* c) {
+    TOP_FOR_WORDS(t, w) {
+        uint32_t bits = 0;
+        for (uint32_t r = t.occ[w]; r; r &= r - 1) {
+            const int b = __ffs(r) - 1;
+            uint64_t s, e;
+            row_times(t, w * 32 + b, s, e);
+            if (expire_due(now, e, idle) || expire_due(now, s, active)) bits |= 1u << b;
+        }
+        bm[w] = bits;                                              // the thread owns the word: every word is written
+        unsigned long long at = warp_reserve(__popc(bits), &c->n);
+        for (uint32_t r = bits; r; r &= r - 1, at++)
+            if (at < cap) list[at] = (uint32_t)(w * 32 + (__ffs(r) - 1));
+    }
+}
+
+// The first slot of every cluster that holds an expiring flow (a set occupancy bit whose cyclic predecessor is clear)
+// into starts.  Reads only: the delete pass changes the occupancy bits the cluster bounds are found from.
+__global__ void __launch_bounds__(256) expire_clusters_kernel(Table t, const uint32_t* __restrict__ bm, uint32_t* __restrict__ starts,
+                                                              ExpireCtr* c) {
+    const uint64_t n_words = (t.mask + 1) >> 5;
+    TOP_FOR_WORDS(t, w) {
+        const uint32_t o = t.occ[w], prev = t.occ[(w + n_words - 1) & (n_words - 1)];   // wraps at the last slot
+        uint32_t take = 0;
+        for (uint32_t r = o & ~((o << 1) | (prev >> 31)); r; r &= r - 1) {
+            const int b = __ffs(r) - 1;
+            for (uint64_t p = w * 32 + b; bit_at(t.occ, p); p = (p + 1) & t.mask)
+                if (bit_at(bm, p)) { take |= 1u << b; break; }
+        }
+        unsigned long long at = warp_reserve(__popc(take), &c->clusters);
+        for (uint32_t r = take; r; r &= r - 1, at++) starts[at] = (uint32_t)(w * 32 + (__ffs(r) - 1));
+    }
+}
+
+// Everything a slot owns: the identity line (key, tag, start mirror), the hot or metric line, the feature lines, the
+// occupancy bit (atomic: neighbouring clusters share bitmap words).  A vacated slot ends all zero, so that a flow created
+// there later inherits nothing.
+__device__ __forceinline__ uint64_t slot_tag(const Table& t, uint64_t s) { return reinterpret_cast<const uint64_t*>(t.ident + s * 8)[5]; }
+__device__ __forceinline__ uint64_t slot_home(const Table& t, uint64_t s) { return top_hash(t, s) & t.mask; }
+__device__ __forceinline__ void move_line(uint4* base, int chunks, uint64_t from, uint64_t to) {
+    for (int k = 0; k < chunks; k++) { base[to * chunks + k] = base[from * chunks + k]; base[from * chunks + k] = make_uint4(0, 0, 0, 0); }
+}
+__device__ __forceinline__ void zero_line(uint4* base, int chunks, uint64_t s) {
+    for (int k = 0; k < chunks; k++) base[s * chunks + k] = make_uint4(0, 0, 0, 0);
+}
+__device__ __forceinline__ void slot_clear(const Table& t, uint64_t s) {
+    zero_line(t.ident, 8, s);
+    if (t.met) zero_line(reinterpret_cast<uint4*>(t.met), kMetLineBytes / 16, s); else zero_line(t.hot, 2, s);
+    if (t.feat_add) zero_line(t.feat_add, kAddState, s);
+    if (t.feat_dns) zero_line(t.feat_dns, kDnsState, s);
+    if (t.feat_drop) zero_line(t.feat_drop, kDropState, s);
+    atomicAnd(&t.occ[s >> 5], ~(1u << (s & 31)));
+}
+__device__ __forceinline__ void slot_move(const Table& t, uint64_t from, uint64_t to) {
+    move_line(t.ident, 8, from, to);
+    if (t.met) move_line(reinterpret_cast<uint4*>(t.met), kMetLineBytes / 16, from, to); else move_line(t.hot, 2, from, to);
+    if (t.feat_add) move_line(t.feat_add, kAddState, from, to);
+    if (t.feat_dns) move_line(t.feat_dns, kDnsState, from, to);
+    if (t.feat_drop) move_line(t.feat_drop, kDropState, from, to);
+    atomicOr(&t.occ[to >> 5], 1u << (to & 31));
+    atomicAnd(&t.occ[from >> 5], ~(1u << (from & 31)));
+}
+
+// One thread per listed cluster.  The cluster's length is read before anything in it changes; within it only this
+// thread writes, and the EMPTY slot after it is never written (a survivor's target lies between its home and itself).
+__global__ void __launch_bounds__(256) expire_compact_kernel(Table t, const uint32_t* __restrict__ bm, const uint32_t* __restrict__ starts,
+                                                             const ExpireCtr* c) {
+    const unsigned long long n = c->clusters;
+    for (unsigned long long i = blockIdx.x * (unsigned long long)blockDim.x + threadIdx.x; i < n; i += (unsigned long long)gridDim.x * blockDim.x) {
+        const uint64_t s = starts[i];
+        uint64_t len = 0;
+        while (bit_at(t.occ, (s + len) & t.mask)) len++;
+        for (uint64_t k = 0; k < len; k++) {
+            const uint64_t p = (s + k) & t.mask;
+            if (bit_at(bm, p)) slot_clear(t, p);
+        }
+        for (uint64_t k = 0; k < len; k++) {                      // survivors in cluster order
+            const uint64_t p = (s + k) & t.mask;
+            if (bit_at(bm, p)) continue;
+            uint64_t q = slot_home(t, p);
+            while (q != p && slot_tag(t, q) != 0) q = (q + 1) & t.mask;
+            if (q != p) slot_move(t, p, q);
+        }
+    }
+}
+
+// A table without an EMPTY slot (FA_F_NO_FULL_CUT with spills): sequential backward-shift deletion on one thread.  An
+// entry at j moves into the hole when its home is not cyclically in (hole, j]; its expire bit moves with it.  Entries
+// move only towards the hole, so no expiring entry lands before the slot being scanned.
+__global__ void expire_full_kernel(Table t, uint32_t* bm) {
+    if (blockIdx.x != 0 || threadIdx.x != 0) return;
+    const uint64_t n_words = (t.mask + 1) >> 5;
+    for (uint64_t w = 0; w < n_words; w++) {
+        while (bm[w]) {
+            const uint64_t i = w * 32 + (__ffs((int)bm[w]) - 1);
+            slot_clear(t, i);
+            bm[w] &= ~(1u << (i & 31));
+            uint64_t hole = i;
+            for (uint64_t j = (i + 1) & t.mask; slot_tag(t, j) != 0; j = (j + 1) & t.mask) {
+                if (((j - slot_home(t, j)) & t.mask) < ((j - hole) & t.mask)) continue;
+                slot_move(t, j, hole);
+                if (bit_at(bm, j)) { bm[j >> 5] &= ~(1u << (j & 31)); bm[hole >> 5] |= 1u << (hole & 31); }
+                hole = j;
+            }
+        }
+    }
+}
+
+__global__ void expire_live_kernel(Counters* ctr, unsigned long long n) {
+    if (blockIdx.x == 0 && threadIdx.x == 0) ctr->live -= n;
+}
+
+// One text for the device and the host emulation (FA_LAUNCH): every kernel loops grid-stride or runs one thread.
+int launch_expire_mark(const Table& t, uint64_t now, uint64_t idle, uint64_t active, const ExpireScratch& s, int sm_count,
+                       cudaStream_t st) {
+    FA_LAUNCH(expire_mark_kernel, sm_count * 8, 256, 0, st, t, now, idle, active, s.bm, s.list, s.cap, s.ctr);
+    return 1;
+}
+
+int launch_expire_emit(const Table& t, bool kmap, const ExpireScratch& s, uint64_t n, uint8_t* out_recs, uint32_t* slot_of_out,
+                       int sm_count, cudaStream_t st) {
+    if (!n) return 0;
+    const uint64_t cap = (uint64_t)sm_count * 8;
+    const uint64_t per_row = (n + 255) / 256, per_lanes = (n * 8 + 255) / 256;     // a thread per row / 8 lanes per row
+    if (kmap) FA_LAUNCH(gather_kmap_kernel, (int)(per_row < cap ? per_row : cap), 256, 0, st, t, s.list, 1u, n, false, out_recs, slot_of_out);
+    else FA_LAUNCH(gather_kernel, (int)(per_lanes < cap ? per_lanes : cap), 256, 0, st, t, s.list, 1u, n, false,
+                   reinterpret_cast<uint4*>(out_recs), slot_of_out);
+    return 1;
+}
+
+int launch_expire_delete(const Table& t, const ExpireScratch& s, uint64_t n, bool full, Counters* ctr, int sm_count,
+                         cudaStream_t st) {
+    if (!n) return 0;
+    if (full) {
+        FA_LAUNCH(expire_full_kernel, 1, 32, 0, st, t, s.bm);
+    } else {
+        FA_LAUNCH(expire_clusters_kernel, sm_count * 8, 256, 0, st, t, s.bm, s.list, s.ctr);
+        FA_LAUNCH(expire_compact_kernel, sm_count * 8, 256, 0, st, t, s.bm, s.list, s.ctr);
+    }
+    FA_LAUNCH(expire_live_kernel, 1, 32, 0, st, ctr, (unsigned long long)n);
+    return full ? 2 : 3;
+}
+
 }  // namespace fa

@@ -40,9 +40,7 @@ namespace fa {
 //   [40] flags (or, u32) | first.eth (u16 @44)           [48] nfs        [56] fe        [64] neth
 //   [72] first.start                  [80] first.end                     [88] latest_drop_cause (u32)
 // additional, extension (no reference analogue): [72] nrtt_min = max ~rtt over rtt != 0 -> smallest non-zero RTT
-constexpr int kAddState = 5;    // uint4 per slot
-constexpr int kDnsState = 8;
-constexpr int kDropState = 6;
+// (kAddState / kDnsState / kDropState, the uint4 per slot, are in kernels.cuh: fa_expire_flows moves these lines)
 
 __device__ __forceinline__ uint64_t ld_u64_unaligned8(const uint8_t* p) { return *reinterpret_cast<const uint64_t*>(p); }
 
@@ -397,15 +395,7 @@ int launch_feature_fold(int kind, const uint8_t* recs, uint32_t n, const Table& 
 }
 #endif  // FA_HOST_EMUL
 
-// ---- eviction: patch the base with the feature effects, emit and clear the feature blocks -----------
-__device__ __forceinline__ void build_base(uint64_t& bs, uint64_t& be, uint32_t& beth, uint64_t nfs, uint64_t fe, uint64_t neth) {
-    // buildBaseFromAdditional (flow_content.go:63-74) with the fold of all samples of one feature
-    const uint64_t s = 0ull - nfs;                       // min non-zero start of the samples, 0 if none
-    if (bs == 0 || (bs > s && s != 0)) bs = s;
-    if (be == 0 || be < fe) be = fe;
-    if (beth == 0 && neth != 0) beth = (uint32_t)(~neth) & 0xFFFFu;
-}
-
+// ---- eviction: patch the base with the feature effects (build_base, kernels.cuh), emit and clear the feature blocks --
 // kClear = false: the fa_top_flows / fa_lookup_flows peek, which emits the same rows and leaves the feature lines as
 // they are; a row whose slot is kNoSlot (a lookup miss) gets zero feature rows and present = 0.
 template <bool kClear = true>

@@ -62,6 +62,20 @@ int launch_full_cut(const uint4* recs, uint32_t n, const Table& table, unsigned 
 // records); slot_of: n u32 scratch
 int launch_feature_fold(int kind, const uint8_t* recs, uint32_t n, const Table& t, uint64_t epoch, uint64_t seq0,
                         uint32_t* slot_of, Counters* ctr, int sm_count, cudaStream_t st);
+// feature lines per slot, in uint4 (layouts in features.cu): additional_metrics, dns_metrics, pkt_drop_metrics
+constexpr int kAddState = 5;
+constexpr int kDnsState = 8;
+constexpr int kDropState = 6;
+#if defined(__CUDACC__) || defined(FA_HOST_EMUL)
+// buildBaseFromAdditional (flow_content.go:63-74) with the fold of all samples of one feature: the eviction's base patch
+// (evict_features_kernel) and the timestamps fa_expire_flows tests
+__device__ __forceinline__ void build_base(uint64_t& bs, uint64_t& be, uint32_t& beth, uint64_t nfs, uint64_t fe, uint64_t neth) {
+    const uint64_t s = 0ull - nfs;                       // min non-zero start of the samples, 0 if none
+    if (bs == 0 || (bs > s && s != 0)) bs = s;
+    if (be == 0 || be < fe) be = fe;
+    if (beth == 0 && neth != 0) beth = (uint32_t)(~neth) & 0xFFFFu;
+}
+#endif
 int launch_evict_features(const Table& t, const uint32_t* slot_of_out, unsigned long long n_out, uint8_t* out_recs,
                           uint8_t* out_dns, uint8_t* out_add, uint8_t* out_drop, unsigned long long* out_rtt_min,
                           uint8_t* out_present, int sm_count, cudaStream_t st);
@@ -108,6 +122,29 @@ int launch_top_flows(const Table& t, bool kmap, const TopMetric& M, uint64_t n, 
 // out_recs (device, n x 144 B; all zero without a flow).  kmap: KERNEL_MAP record layout.  Nothing in `t` changes.
 int launch_lookup_flows(const Table& t, bool kmap, const uint64_t* keys, uint64_t n, uint32_t* slots, uint8_t* found,
                         unsigned long long* hits, uint8_t* out_recs, int sm_count, cudaStream_t st);
+
+// fa_expire_flows (evict.cu): remove the flows past an idle or active timeout and compact their probe chains in place.
+struct ExpireCtr {
+    unsigned long long n;                          // expiring flows (mark)
+    unsigned long long clusters;                   // clusters that hold one of them (the cluster pass)
+};
+struct ExpireScratch {
+    uint32_t* bm;                                  // expire bitmap, 1 bit per slot (every word written by the mark)
+    uint32_t* list;                                // cap entries: the expiring slots; after the gather, the cluster starts
+    uint64_t cap;
+    ExpireCtr* ctr;                                // zeroed before the mark
+};
+// Mark: the expire bitmap, the expiring slots (the first cap of them) and their count in s.ctr->n.  Reads only.
+int launch_expire_mark(const Table& t, uint64_t now, uint64_t idle, uint64_t active, const ExpireScratch& s, int sm_count,
+                       cudaStream_t st);
+// Emit: rows of the n listed slots into out_recs (device, n x 144 B), their slots into slot_of_out (optional, for the
+// feature pass).  kmap: KERNEL_MAP record layout.
+int launch_expire_emit(const Table& t, bool kmap, const ExpireScratch& s, uint64_t n, uint8_t* out_recs, uint32_t* slot_of_out,
+                       int sm_count, cudaStream_t st);
+// Delete the n marked flows with every line they own, move the survivors of their clusters back towards their home slots,
+// and take n off ctr->live.  full: the table has no EMPTY slot (one thread, backward-shift deletion).
+int launch_expire_delete(const Table& t, const ExpireScratch& s, uint64_t n, bool full, Counters* ctr, int sm_count,
+                         cudaStream_t st);
 
 // sketches
 int launch_cms_query(const SketchParams& sk, const uint4* keys, uint32_t n, unsigned long long* est, cudaStream_t st);

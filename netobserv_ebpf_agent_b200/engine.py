@@ -200,6 +200,24 @@ class FlowAggEngine:
         check(lib().fa_lookup_flows(self._h, k.ctypes.data, m, C.byref(o), found.ctypes.data, C.byref(got)))
         return out[:m], dns[:m], add[:m], drops[:m], rmin[:m], pres[:m], found[:m]
 
+    def expire_flows(self, mono_now_ns, idle_timeout_ns=0, active_timeout_ns=0, cap=None):
+        """Lookup-and-delete only the flows past the idle timeout (no record for idle_timeout_ns) or the active timeout
+        (open for active_timeout_ns), 0 = that timer is off; every other flow stays live -> the six arrays of evict_ex
+        (records, dns, additional, pkt_drops, rtt_min, present) for the expired flows.
+        cap: output capacity in flows (default: the live count right now)."""
+        from ._lib import EvictOut
+        if cap is None:
+            cap = max(self.live_flows(), 1)
+        out, dns, add = np.zeros((cap, REC_BYTES), np.uint8), np.zeros((cap, 64), np.uint8), np.zeros((cap, 32), np.uint8)
+        drops, rmin, pres = np.zeros((cap, 32), np.uint8), np.zeros(cap, np.uint64), np.zeros(cap, np.uint8)
+        o = EvictOut(records=out.ctypes.data, dns=dns.ctypes.data, additional=add.ctypes.data, pkt_drops=drops.ctypes.data,
+                     rtt_min=rmin.ctypes.data, present=pres.ctypes.data)
+        got = C.c_size_t(0)
+        check(lib().fa_expire_flows(self._h, int(mono_now_ns), int(idle_timeout_ns), int(active_timeout_ns), C.byref(o), cap,
+                                    C.byref(got)))
+        g = got.value
+        return out[:g], dns[:g], add[:g], drops[:g], rmin[:g], pres[:g]
+
     def read_spilled(self, cap=131072):
         """KERNEL_MAP mode with FA_F_RINGBUF_FALLBACK: the single-packet records that could not enter the full map
         (the batched equivalent of reading the direct_flows ring buffer) -> (n,144) uint8 array."""
