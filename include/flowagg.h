@@ -452,6 +452,44 @@ int fa_lookup_flows(fa_engine* e, const void* keys, size_t n, const fa_evict_out
 int fa_expire_flows(fa_engine* e, uint64_t mono_now_ns, uint64_t idle_timeout_ns, uint64_t active_timeout_ns,
                     const fa_evict_out* out, size_t cap, size_t* n_out);
 
+/* One group of fa_group_flows, 88 bytes. */
+typedef struct fa_flow_group {
+    fa_flow_id key;                  /*  0 the group: a flow key AND key_mask (byte 39 = 0) */
+    uint64_t   flows;                /* 40 live flows in the group (feature-only flows included) */
+    uint64_t   bytes;                /* 48 sum of the rows' bytes (record offset 56), mod 2^64 */
+    uint64_t   packets;              /* 56 sum of the rows' u32 packets (record offset 64), in 64 bits: no wrap */
+    uint64_t   start_mono_time_ts;   /* 64 smallest non-zero row start; 0 if every row's start is 0 */
+    uint64_t   end_mono_time_ts;     /* 72 largest row end */
+    uint16_t   flags;                /* 80 OR of the rows' TCP flags (record offset 70) */
+    uint8_t    pad_[6];              /* 82 always 0 */
+} fa_flow_group;
+
+/* Roll-ups of the live flows by a key mask (per subnet, per service port, per protocol, fan-out of one host, totals of
+ * the window), on the device, WITHOUT removing or changing anything (no reference analogue: downstream of the agent
+ * the same group-by runs on the host over evicted flows).
+ *   Group:  a flow belongs to the group of its 40-byte key ANDed with key_mask (host memory, 40 bytes; byte 39 is
+ *           ignored and the group key's byte 39 is 0).  IPv4 keys are ::ffff:a.b.c.d, so an IPv4 /p is a mask of 96 + p
+ *           bits over the 16 address bytes.  An all-zero mask gives one group (the window's totals), an all-ones mask
+ *           one group per flow.
+ *   Values: "the row" of a flow is the row fa_evict_ex would return for it now, in both modes, base patch of feature-only
+ *           flows included (their start and end come from the feature lines; their bytes, packets and flags are 0, and
+ *           they count in `flows`).  In KERNEL_MAP mode packets and bytes are those of the first-seen interface, as that
+ *           row carries them.  Sums and extremes as documented in fa_flow_group.
+ *   Output: every group exactly once, in unspecified order, into `out` (host pageable / pinned or device memory; device
+ *           memory 8-byte aligned), room for cap rows.  *n_groups = the number of groups.
+ *   Nothing changes: the table, the feature lines, the live count, the sketch, the DNS correlation table and the
+ *           fallback ring are as before, and a later eviction returns what it would have returned without the call; in
+ *           fa_stats only kernel_launches and d2h_bytes move.
+ *   Runs on the engine stream after every queued fold, under the engine lock, and returns when `out` is complete.
+ *   FA_F_NONBLOCKING_EVICT: groups the live table only, not a retired table still being evicted.  The fallback ring
+ *   (fa_read_spilled) is not part of the table.  Device scratch, allocated on first use and grown with the live count:
+ *   a group table of the smallest power of two >= max(1024, 4/3 x live) slots of 96 B + 4 B (about 1.6 GB at 10^7
+ *   live flows), and 88 B per group of staging for a host `out`.
+ *   FA_E_2BIG: more than cap groups; *n_groups = the exact count and nothing is written to `out`.  `out` may be NULL
+ *   when cap == 0: a count query.
+ *   FA_E_INVAL: null engine / key_mask / n_groups, out == NULL with cap > 0, device `out` not 8-byte aligned. */
+int fa_group_flows(fa_engine* e, const uint8_t key_mask[40], fa_flow_group* out, size_t cap, size_t* n_groups);
+
 /* Lookup-and-RESET (no reference analogue; building block of the multi-GPU local combiner, the counterpart of
  * the reference folding its per-CPU maps in user space, pkg/tracer/tracer.go:1159-1187): every flow that received
  * records since the previous drain is written to out_records (device memory, cap x 144 B) as a partial flow record

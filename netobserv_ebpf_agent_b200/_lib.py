@@ -2,6 +2,8 @@
 import ctypes as C
 import os
 
+import numpy as np
+
 HERE = os.path.dirname(os.path.abspath(__file__))
 REC_BYTES, ID_BYTES, DNS_BYTES, ADD_BYTES, DNSREC_BYTES, ADDREC_BYTES = 144, 40, 64, 32, 104, 72
 
@@ -58,6 +60,11 @@ class PbParams(C.Structure):
 
 FA_PB_WRAP_ENTRIES = 1
 
+# fa_flow_group (88 bytes), include/flowagg.h
+GROUP_DTYPE = np.dtype([("key", "u1", 40), ("flows", "<u8"), ("bytes", "<u8"), ("packets", "<u8"),
+                        ("start_mono_time_ts", "<u8"), ("end_mono_time_ts", "<u8"), ("flags", "<u2"), ("pad_", "u1", 6)])
+assert GROUP_DTYPE.itemsize == 88
+
 
 class GenParams(C.Structure):
     _fields_ = [("seed", C.c_uint64), ("n_keys", C.c_uint64), ("dist", C.c_uint32), ("zipf_s_milli", C.c_uint32),
@@ -84,6 +91,7 @@ SIGNATURES = {
                                   C.POINTER(C.c_size_t)]),
     "fa_expire_flows": (C.c_int, [C.c_void_p, C.c_uint64, C.c_uint64, C.c_uint64, C.POINTER(EvictOut), C.c_size_t,
                                   C.POINTER(C.c_size_t)]),
+    "fa_group_flows": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_size_t, C.POINTER(C.c_size_t)]),
     "fa_evict": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_size_t,
                            C.POINTER(C.c_size_t)]),
     "fa_drain_active": (C.c_int, [C.c_void_p, C.c_void_p, C.c_size_t, C.POINTER(C.c_size_t)]),

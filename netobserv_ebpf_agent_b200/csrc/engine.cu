@@ -160,6 +160,10 @@ struct fa_engine {
     Staging expire_stage;                     // fa_expire_flows: under `mu`
     fa::ExpireScratch expire{};               // fa_expire_flows: expire bitmap, slot list (cap entries), counters
     fa::ExpireCtr* h_expire_ctr = nullptr;    // pinned
+    fa::GroupScratch group{};                 // fa_group_flows, under `mu`: group table (all zero between calls), list, counters
+    fa::GroupCtr* h_group_ctr = nullptr;      // pinned
+    uint8_t* d_group_out = nullptr;           // ... and its staging of host-bound rows, group_out_cap rows
+    uint64_t group_out_cap = 0;
     uint32_t* d_slot_of = nullptr;            // per-sample slot scratch of the feature folds
     uint64_t feat_seq[3] = {0, 0, 0};         // running sample numbers (additional, dns, packet drops)
     uint32_t* d_route_tmp = nullptr; unsigned long long* d_route_counts = nullptr;
@@ -687,6 +691,8 @@ void fa_destroy(fa_engine* e) {
     if (e->h_lookup_hits) cudaFreeHost(e->h_lookup_hits);
     free_staging(&e->expire_stage); cudaFree(e->expire.bm); cudaFree(e->expire.list); cudaFree(e->expire.ctr);
     if (e->h_expire_ctr) cudaFreeHost(e->h_expire_ctr);
+    cudaFree(e->group.tab); cudaFree(e->group.list); cudaFree(e->group.ctr); cudaFree(e->d_group_out);
+    if (e->h_group_ctr) cudaFreeHost(e->h_group_ctr);
     cudaFree(e->sk.cms); cudaFree(e->sk.hll);
     cudaFree(e->dnsc.tab); cudaFree(e->dnsc_spare); cudaFree(e->dnsc.ctr); cudaFreeHost(e->h_dnsc_ctr);
     cudaFree(e->d_dnsc_state); cudaFree(e->d_dnsc_samples); cudaFree(e->d_dnsc_out); cudaFree(e->d_dnsc_warps);
@@ -1234,6 +1240,79 @@ int fa_expire_flows(fa_engine* e, uint64_t mono_now_ns, uint64_t idle_timeout_ns
     e->st.d2h_bytes += d2h;
     *n_out = (size_t)n;
     return FA_OK;
+}
+
+// Exact roll-ups of the live flows by a key mask, read in place (evict.cu: launch_group_*), on the engine stream after
+// the queued folds: the scan folds every live flow into the group table and lists the groups, the host reads their
+// count (one wait), then one pass writes the listed groups' rows (device `out` in place, host `out` through the group
+// staging) and zeroes their slots, or only zeroes them when the rows are not wanted (FA_E_2BIG).  Either way the group
+// table is all zero again for the next call.  Nothing of the flow table or the counters is written.
+static int grow_group_out(fa_engine* e, uint64_t n) {
+    if (e->group_out_cap >= n) return FA_OK;
+    cudaFree(e->d_group_out); e->d_group_out = nullptr; e->group_out_cap = 0;
+    const uint64_t want = std::max<uint64_t>(n, std::min<uint64_t>(e->slots, 2 * n));
+    CU(cudaMalloc(&e->d_group_out, want * fa::kGroupRowBytes));
+    e->group_out_cap = want;
+    return FA_OK;
+}
+
+int fa_group_flows(fa_engine* e, const uint8_t key_mask[40], fa_flow_group* out, size_t cap, size_t* n_groups) {
+    if (n_groups) *n_groups = 0;
+    if (!e || !key_mask || !n_groups || (!out && cap)) return fail(FA_E_INVAL, "fa_group_flows: null argument");
+    std::lock_guard<std::mutex> lk(e->mu);
+    CU(cudaSetDevice(e->device));
+    const bool out_dev = out && classify(out) == PTR_DEVICE;
+    if (out_dev && (reinterpret_cast<uintptr_t>(out) & 7))
+        return fail(FA_E_INVAL, "fa_group_flows: device out must be 8-byte aligned");
+    if (int rc = sync_counters(e)) return rc;          // the queued folds finish; exact live count
+    const uint64_t live = e->live_known;
+    if (live == 0) return FA_OK;
+    cudaStream_t st = e->stream;
+    fa::GroupMask m;
+    memcpy(m.w, key_mask, fa::kKeyBytes);
+    m.w[4] &= 0x00FFFFFFFFFFFFFFull;                   // byte 39 (padding) is ignored
+    uint64_t slots = 1024;                             // load factor <= 3/4: groups never outnumber the live flows
+    while (slots < (4 * live + 2) / 3) slots <<= 1;
+    if (!e->group.tab || e->group.mask + 1 < slots) {
+        cudaFree(e->group.tab); cudaFree(e->group.list);
+        e->group.tab = nullptr; e->group.list = nullptr; e->group.mask = 0;
+        CU(cudaMalloc(&e->group.tab, slots * fa::kGroupSlotWords * 8));
+        CU(cudaMalloc(&e->group.list, slots * 4));
+        CU(cudaMemsetAsync(e->group.tab, 0, slots * fa::kGroupSlotWords * 8, st));
+        e->group.mask = slots - 1;
+    }
+    if (!e->group.ctr) CU(cudaMalloc(&e->group.ctr, sizeof(fa::GroupCtr)));
+    if (!e->h_group_ctr) CU(cudaHostAlloc(&e->h_group_ctr, sizeof(fa::GroupCtr), cudaHostAllocDefault));
+    const fa::GroupScratch s = e->group;
+    CU(cudaMemsetAsync(s.ctr, 0, sizeof(fa::GroupCtr), st));
+    uint64_t launched = fa::launch_group_scan(e->table, m, s, e->sm_count, st);
+    CU(cudaGetLastError());
+    CU(cudaMemcpyAsync(e->h_group_ctr, s.ctr, sizeof(fa::GroupCtr), cudaMemcpyDeviceToHost, st));
+    CU(cudaStreamSynchronize(st));
+    const uint64_t n = e->h_group_ctr->n;
+    int rc = FA_OK;
+    if (e->h_group_ctr->lost || n > live)
+        rc = fail(FA_E_CUDA, "fa_group_flows: %llu groups of %llu live flows, %llu folds without a slot", (unsigned long long)n,
+                  (unsigned long long)live, e->h_group_ctr->lost);
+    else if (n > cap)
+        rc = fail(FA_E_2BIG, "fa_group_flows: capacity %zu < %llu groups", cap, (unsigned long long)n);
+    uint64_t* rows = nullptr;
+    if (rc == FA_OK) {
+        if (out_dev) rows = reinterpret_cast<uint64_t*>(out);
+        else if ((rc = grow_group_out(e, n)) == FA_OK) rows = reinterpret_cast<uint64_t*>(e->d_group_out);
+    }
+    launched += fa::launch_group_emit(s, std::min<uint64_t>(n, s.mask + 1), rows, e->sm_count, st);   // rows == nullptr: clear only
+    CU(cudaGetLastError());
+    uint64_t d2h = 0;
+    if (rows && !out_dev) {
+        CU(cudaMemcpyAsync(out, rows, n * fa::kGroupRowBytes, cudaMemcpyDeviceToHost, st));
+        d2h = n * fa::kGroupRowBytes;
+    }
+    CU(cudaStreamSynchronize(st));
+    e->st.kernel_launches += launched;
+    e->st.d2h_bytes += d2h;
+    if (rc == FA_OK || rc == FA_E_2BIG) *n_groups = (size_t)n;
+    return rc;
 }
 
 // Emit and reset the flows touched since the last drain into out_records_dev.  The count goes to *n_dev_out (device

@@ -623,4 +623,160 @@ int launch_expire_delete(const Table& t, const ExpireScratch& s, uint64_t n, boo
     return full ? 2 : 3;
 }
 
+// ---- fa_group_flows: exact roll-ups of the live flows by a key mask, without removing or changing anything --------
+// Scan (bitmap-driven, like expire_mark_kernel): each live flow's masked key and its row values (bytes, packets and
+// flags from the hot or metric line, start / end from row_times, so with the eviction's feature patch).  The lanes of
+// a warp take one flow each per round; the lanes with an equal masked key (every one of its ten 32-bit words: distinct
+// keys can share a premix) form a peer set, and one leader per set folds the set's sum into the group table.  Emit /
+// clear: one thread per listed group writes its row and zeroes its slot.
+//
+// Group-table slot (12 u64): [0, 5) the group key, [5] state (0 EMPTY, kGroupWriting, kGroupPublished), [6] flows,
+// [7] bytes, [8] packets, [9] nstart = 0 - start (max: the smallest non-zero start, 0 if none), [10] end (max),
+// [11] flags (or).  Every accumulator is commutative with identity 0, so the result does not depend on the order of
+// the updates, and a slot that was never claimed or was emitted is all zero.
+constexpr unsigned long long kGroupWriting = 1ull, kGroupPublished = 2ull;
+
+struct GroupVals { uint64_t bytes, packets, nstart, end; uint32_t flags; };
+
+// The fields of the row fa_evict_ex would return for `slot` now that fa_flow_group sums (packets widened to 64 bits).
+__device__ __forceinline__ GroupVals group_row(const Table& t, uint64_t slot) {
+    GroupVals v;
+    uint64_t s, e;
+    row_times(t, slot, s, e);
+    v.nstart = 0ull - s; v.end = e;
+    if (t.met) {
+        const uint8_t* M = t.met + slot * kMetLineBytes;
+        v.bytes = km_ld64(M + KM_BYTES); v.packets = km_ld32(M + KM_PACKETS); v.flags = km_ld16(M + KM_FLAGS);
+    } else {
+        const uint64_t* H = reinterpret_cast<const uint64_t*>(t.hot + slot * 2);
+        v.bytes = H[0]; v.packets = (uint32_t)H[3]; v.flags = (uint32_t)(H[3] >> 32) & 0xFFFFu;
+    }
+    return v;
+}
+
+__device__ __forceinline__ void group_add(unsigned long long* G, uint64_t flows, const GroupVals& v) {
+    red_add_u64(G + 6, flows);
+    if (v.bytes) red_add_u64(G + 7, v.bytes);
+    if (v.packets) red_add_u64(G + 8, v.packets);
+    if (v.nstart) red_max_u64(G + 9, v.nstart);
+    if (v.end) red_max_u64(G + 10, v.end);
+    if (v.flags) red_or_u64(G + 11, v.flags);
+}
+
+// Fold `flows` flows with the summed values v into the group of key k, creating it the way K1 creates a flow: claim an
+// EMPTY slot by CAS on its state, write the key, fence, publish; a walk that meets a slot being written waits for the
+// publish.  Linear probing from the key's slot hash, at most every slot once.  false: no slot found (the table always
+// has more slots than the live flows, so this does not happen).
+__device__ __forceinline__ bool group_fold(const GroupScratch& s, const uint64_t k[5], uint64_t flows, const GroupVals& v) {
+    uint64_t slot = slot_hash(key_premix(k[0], k[1], k[2], k[3], k[4])) & s.mask;
+    for (uint64_t probes = 0; probes <= s.mask; probes++, slot = (slot + 1) & s.mask) {
+        unsigned long long* G = s.tab + slot * kGroupSlotWords;
+        unsigned long long state = ld_cg_u64(G + 5);
+        if (state == 0ull) {
+            state = atomicCAS(G + 5, 0ull, kGroupWriting);
+            if (state == 0ull) {
+#pragma unroll
+                for (int w = 0; w < 5; w++) G[w] = k[w];
+                __threadfence();
+                atomicCAS(G + 5, kGroupWriting, kGroupPublished);
+                s.list[atomicAdd(&s.ctr->n, 1ull)] = (uint32_t)slot;     // one group per slot: the list cannot overflow
+                group_add(G, flows, v);
+                return true;
+            }
+        }
+        // a volatile load: the compiler may not assume the state stays the same and drop the wait
+        while (state == kGroupWriting) state = *reinterpret_cast<volatile unsigned long long*>(G + 5);
+        __threadfence();
+        unsigned long long diff = 0;
+#pragma unroll
+        for (int w = 0; w < 5; w++) diff |= ld_cg_u64(G + w) ^ k[w];
+        if (diff == 0) {
+            group_add(G, flows, v);
+            return true;
+        }
+    }
+    return false;
+}
+
+__global__ void __launch_bounds__(256) group_scan_kernel(Table t, GroupMask m, GroupScratch s) {
+    const int lane = threadIdx.x & 31;
+    TOP_FOR_WORDS(t, w) {
+        uint32_t r = t.occ[w];
+        while (__any_sync(0xFFFFFFFFu, r != 0u)) {             // converged rounds: at most one flow per lane
+            const bool have = r != 0u;
+            uint64_t k[5] = {0, 0, 0, 0, 0};
+            GroupVals v = {0, 0, 0, 0, 0u};                       // lanes without a flow hold the identity
+            if (have) {
+                const uint64_t slot = w * 32 + (__ffs(r) - 1);
+                r &= r - 1;
+                const uint64_t* L = reinterpret_cast<const uint64_t*>(t.ident) + slot * (kIdentBytes / 8);
+#pragma unroll
+                for (int i = 0; i < 5; i++) k[i] = L[i] & m.w[i];
+                v = group_row(t, slot);
+            }
+            const uint32_t active = __ballot_sync(0xFFFFFFFFu, have);
+            uint32_t peers = active;
+#pragma unroll
+            for (int i = 0; i < 5; i++) {
+                peers &= __match_any_sync(0xFFFFFFFFu, (uint32_t)k[i]);
+                peers &= __match_any_sync(0xFFFFFFFFu, (uint32_t)(k[i] >> 32));
+            }
+            if (!have) peers = 0u;
+            const int np = __popc(peers);
+            if (__any_sync(0xFFFFFFFFu, np > 1)) {
+                if (__all_sync(0xFFFFFFFFu, !have || peers == active)) {
+                    // one peer set holds every flow of the round (a coarse mask): a butterfly over the warp
+                    for (int d = 16; d > 0; d >>= 1) {
+                        const uint64_t b = __shfl_sync(0xFFFFFFFFu, v.bytes, lane ^ d), p = __shfl_sync(0xFFFFFFFFu, v.packets, lane ^ d);
+                        const uint64_t ns = __shfl_sync(0xFFFFFFFFu, v.nstart, lane ^ d), e = __shfl_sync(0xFFFFFFFFu, v.end, lane ^ d);
+                        const uint32_t f = __shfl_sync(0xFFFFFFFFu, v.flags, lane ^ d);
+                        v.bytes += b; v.packets += p; v.nstart = ns > v.nstart ? ns : v.nstart; v.end = e > v.end ? e : v.end; v.flags |= f;
+                    }
+                } else {
+                    // several sets: step q, every lane reads the q-th lane of its own set (the leader is lane 0 of it)
+                    GroupVals a = v;
+                    const int most = (int)__reduce_max_sync(0xFFFFFFFFu, (unsigned)np);
+                    for (int q = 1; q < most; q++) {
+                        const int src = q < np ? (int)__fns(peers, 0, q + 1) : lane;
+                        const uint64_t b = __shfl_sync(0xFFFFFFFFu, v.bytes, src), p = __shfl_sync(0xFFFFFFFFu, v.packets, src);
+                        const uint64_t ns = __shfl_sync(0xFFFFFFFFu, v.nstart, src), e = __shfl_sync(0xFFFFFFFFu, v.end, src);
+                        const uint32_t f = __shfl_sync(0xFFFFFFFFu, v.flags, src);
+                        if (q < np) { a.bytes += b; a.packets += p; a.nstart = ns > a.nstart ? ns : a.nstart; a.end = e > a.end ? e : a.end; a.flags |= f; }
+                    }
+                    v = a;
+                }
+            }
+            if (have && lane == __ffs(peers) - 1 && !group_fold(s, k, (uint64_t)np, v)) atomicAdd(&s.ctr->lost, 1ull);
+        }
+    }
+}
+
+// Row i from the i-th listed group (out != nullptr), then its slot back to all zero.
+__global__ void __launch_bounds__(256) group_emit_kernel(GroupScratch s, unsigned long long n, uint64_t* __restrict__ out) {
+    for (unsigned long long i = blockIdx.x * (unsigned long long)blockDim.x + threadIdx.x; i < n; i += (unsigned long long)gridDim.x * blockDim.x) {
+        unsigned long long* G = s.tab + (uint64_t)s.list[i] * kGroupSlotWords;
+        if (out) {
+            uint64_t* O = out + i * (kGroupRowBytes / 8);
+            for (int w = 0; w < 5; w++) O[w] = G[w];
+            O[5] = G[6]; O[6] = G[7]; O[7] = G[8];              // flows, bytes, packets
+            O[8] = 0ull - G[9]; O[9] = G[10];                   // start (0 stays 0), end
+            O[10] = G[11] & 0xFFFFull;                          // flags, pad_ = 0
+        }
+        for (int w = 0; w < kGroupSlotWords; w++) G[w] = 0ull;
+    }
+}
+
+// One text for the device and the host emulation (FA_LAUNCH): both kernels loop grid-stride.
+int launch_group_scan(const Table& t, const GroupMask& m, const GroupScratch& s, int sm_count, cudaStream_t st) {
+    FA_LAUNCH(group_scan_kernel, sm_count * 8, 256, 0, st, t, m, s);
+    return 1;
+}
+
+int launch_group_emit(const GroupScratch& s, uint64_t n, uint64_t* out, int sm_count, cudaStream_t st) {
+    if (!n) return 0;
+    const uint64_t cap = (uint64_t)sm_count * 8, per_row = (n + 255) / 256;
+    FA_LAUNCH(group_emit_kernel, (int)(per_row < cap ? per_row : cap), 256, 0, st, s, (unsigned long long)n, out);
+    return 1;
+}
+
 }  // namespace fa

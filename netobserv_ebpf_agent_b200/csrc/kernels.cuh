@@ -146,6 +146,27 @@ int launch_expire_emit(const Table& t, bool kmap, const ExpireScratch& s, uint64
 int launch_expire_delete(const Table& t, const ExpireScratch& s, uint64_t n, bool full, Counters* ctr, int sm_count,
                          cudaStream_t st);
 
+// fa_group_flows (evict.cu): roll the live flows up by a key mask in an open-addressed group table (slot layout in
+// evict.cu), list the groups, then emit or clear them.
+constexpr int kGroupSlotWords = 12;                // one group-table slot: 12 u64 = 96 B
+constexpr int kGroupRowBytes = 88;                 // one fa_flow_group row
+struct GroupCtr {
+    unsigned long long n;                          // groups created: the list cursor
+    unsigned long long lost;                       // folds whose walk met neither their group nor an EMPTY slot (never)
+};
+struct GroupScratch {
+    unsigned long long* tab;                       // (mask + 1) slots, all zero between calls
+    uint32_t* list;                                // mask + 1 entries: the slot of every group, in creation order
+    uint64_t mask;                                 // slots - 1 (slots: a power of two > 4/3 x the live flows)
+    GroupCtr* ctr;                                 // zeroed before the scan
+};
+struct GroupMask { uint64_t w[5]; };               // the 40-byte key mask as five little-endian words, byte 39 clear
+// Scan: fold every live flow of `t` into the group of its masked key (created when absent).  Reads `t` only.
+int launch_group_scan(const Table& t, const GroupMask& m, const GroupScratch& s, int sm_count, cudaStream_t st);
+// Emit the n listed groups as fa_flow_group rows into out (device, 8-byte aligned; nullptr: write nothing) and zero
+// their slots, so that the table is all zero again.
+int launch_group_emit(const GroupScratch& s, uint64_t n, uint64_t* out, int sm_count, cudaStream_t st);
+
 // sketches
 int launch_cms_query(const SketchParams& sk, const uint4* keys, uint32_t n, unsigned long long* est, cudaStream_t st);
 int launch_hll_pack(const SketchParams& sk, uint8_t* out_regs, cudaStream_t st);

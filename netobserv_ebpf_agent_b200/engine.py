@@ -39,6 +39,33 @@ FILTER_CIDR_DTYPE = np.dtype([("ip", "u1", 16), ("prefix_len", "<u4")])
 assert FILTER_RULE_DTYPE.itemsize == 64 and FILTER_CIDR_DTYPE.itemsize == 20
 
 
+def _prefix_bytes(bits):
+    """The 16 mask bytes of a prefix of `bits` bits (0..128) over a 16-byte address field."""
+    assert 0 <= bits <= 128, bits
+    m = np.zeros(16, np.uint8)
+    m[: bits // 8] = 0xFF
+    if bits % 8:
+        m[bits // 8] = (0xFF00 >> (bits % 8)) & 0xFF
+    return m
+
+
+def group_mask(src_prefix=0, dst_prefix=0, src_port=False, dst_port=False, proto=False, icmp=False):
+    """The 40-byte key mask of FlowAggEngine.group_flows / fa_group_flows: the first src_prefix / dst_prefix bits of the
+    16-byte addresses (IPv4 keys are ::ffff:a.b.c.d, so an IPv4 /24 is 96 + 24 = 120), the ports, the transport
+    protocol, the ICMP type and code."""
+    m = np.zeros(40, np.uint8)
+    m[0:16], m[16:32] = _prefix_bytes(src_prefix), _prefix_bytes(dst_prefix)
+    if src_port:
+        m[32:34] = 0xFF
+    if dst_port:
+        m[34:36] = 0xFF
+    if proto:
+        m[36] = 0xFF
+    if icmp:
+        m[37:39] = 0xFF
+    return m
+
+
 class FlowAggEngine:
     """One engine == one GPU flow cache (the reference's aggregated_flows map + Accounter)."""
 
@@ -217,6 +244,19 @@ class FlowAggEngine:
                                     C.byref(got)))
         g = got.value
         return out[:g], dns[:g], add[:g], drops[:g], rmin[:g], pres[:g]
+
+    def group_flows(self, mask, cap=None):
+        """Roll the live flows up by a 40-byte key mask (group_mask) without changing anything -> a GROUP_DTYPE array,
+        one row per group, in unspecified order.  cap: room in groups (default: the live count right now)."""
+        from ._lib import GROUP_DTYPE
+        m = np.ascontiguousarray(mask, dtype=np.uint8).reshape(-1)
+        assert m.size == 40, m.size
+        if cap is None:
+            cap = max(self.live_flows(), 1)
+        out = np.zeros(cap, GROUP_DTYPE)
+        got = C.c_size_t(0)
+        check(lib().fa_group_flows(self._h, m.ctypes.data, out.ctypes.data, cap, C.byref(got)))
+        return out[: got.value]
 
     def read_spilled(self, cap=131072):
         """KERNEL_MAP mode with FA_F_RINGBUF_FALLBACK: the single-packet records that could not enter the full map
