@@ -490,6 +490,53 @@ typedef struct fa_flow_group {
  *   FA_E_INVAL: null engine / key_mask / n_groups, out == NULL with cap > 0, device `out` not 8-byte aligned. */
 int fa_group_flows(fa_engine* e, const uint8_t key_mask[40], fa_flow_group* out, size_t cap, size_t* n_groups);
 
+/* The per-flow value fa_histogram_flows bins, and which flows have one. */
+#define FA_HIST_BYTES        0u  /* record bytes (offset 56): every flow */
+#define FA_HIST_PACKETS      1u  /* record packets (offset 64, u32): every flow */
+#define FA_HIST_DURATION     2u  /* end - start of the row (offsets 48 - 40), 0 if end < start: flows with start != 0 */
+#define FA_HIST_RTT          3u  /* additional.flow_rtt (ns): flows whose value is != 0       (needs FA_F_ENABLE_RTT) */
+#define FA_HIST_DNS_LATENCY  4u  /* dns.latency (ns): flows with a DNS block and dns.id != 0  (needs FA_F_ENABLE_DNS) */
+#define FA_HIST_MAX_BOUNDS   63u
+#define FA_HIST_ROW_BYTES(n_bounds) (80u + 8u * ((n_bounds) + 1u))
+
+typedef struct fa_hist_row {     /* header of one row; n_bounds + 1 u64 bucket counts follow at offset 80 */
+    fa_flow_id key;              /*  0 the group: flow key AND key_mask, byte 39 = 0 (as fa_flow_group.key) */
+    uint64_t   flows;            /* 40 live flows in the group (as fa_flow_group.flows) */
+    uint64_t   count;            /* 48 flows of the group that have a value (= the sum of the bucket counts) */
+    uint64_t   sum;              /* 56 sum of those values, mod 2^64 */
+    uint64_t   min, max;         /* 64, 72 smallest / largest value; 0 when count == 0 */
+} fa_hist_row;
+
+/* Per-group histograms of one per-flow value over the live flows (flow size, duration, RTT or DNS latency per subnet,
+ * per service, per server), on the device, WITHOUT removing or changing anything (no reference analogue: downstream of
+ * the agent RTT and DNS latency are published as Prometheus histograms with fixed `le` buckets).
+ *   Group:  as fa_group_flows with the same key_mask: the same groups, keys and flow counts.
+ *   Value:  `value` (FA_HIST_*) of the row fa_evict_ex would return for the flow now, in both modes, base patch of
+ *           feature-only flows included.  A flow without the value (the decoder's presence rules: no start, a zero RTT,
+ *           no DNS block or a zero DNS id, as for an IPsec-only or an errno-only sample) counts in `flows` only.
+ *   Buckets: bounds (host memory) holds n_bounds Prometheus `le` upper bounds, strictly increasing, 1 <= n_bounds <=
+ *           FA_HIST_MAX_BOUNDS.  Bucket 0 counts the values v <= bounds[0], bucket i < n_bounds those with
+ *           bounds[i-1] < v <= bounds[i], bucket n_bounds (+Inf) those above bounds[n_bounds-1].  Per bucket, not
+ *           cumulative.
+ *   Output: every group exactly once, in unspecified order, into `out` (host pageable / pinned or device memory; device
+ *           memory 8-byte aligned), room for cap rows of FA_HIST_ROW_BYTES(n_bounds) bytes.  *n_groups = the number of
+ *           groups.
+ *   Nothing changes: the table, the feature lines, the live count, the sketch, the DNS correlation table, the fallback
+ *           ring and fa_group_flows' group table are as before, and a later eviction returns what it would have returned
+ *           without the call; in fa_stats only kernel_launches and d2h_bytes move.
+ *   Runs on the engine stream after every queued fold, under the engine lock, and returns when `out` is complete.
+ *   FA_F_NONBLOCKING_EVICT: bins the live table only, not a retired table still being evicted.  The fallback ring
+ *   (fa_read_spilled) is not part of the table.  Device scratch, allocated on first use and grown with the live count:
+ *   fa_group_flows' group table plus 4 B per slot of it, and FA_HIST_ROW_BYTES(n_bounds) per group of staging for a
+ *   host `out` (592 B at 63 bounds: an all-ones mask over 10^7 live flows stages about 5.9 GB; cap bounds it).
+ *   FA_E_2BIG: more than cap groups; *n_groups = the exact count and nothing is written to `out`.  `out` may be NULL
+ *   when cap == 0: a count query.
+ *   FA_E_INVAL: null engine / key_mask / bounds / n_groups, out == NULL with cap > 0, device `out` not 8-byte aligned,
+ *   an unknown value, n_bounds == 0 or > FA_HIST_MAX_BOUNDS, bounds not strictly increasing, FA_HIST_RTT without
+ *   FA_F_ENABLE_RTT, FA_HIST_DNS_LATENCY without FA_F_ENABLE_DNS (nothing changes). */
+int fa_histogram_flows(fa_engine* e, const uint8_t key_mask[40], uint32_t value, const uint64_t* bounds, uint32_t n_bounds,
+                       void* out, size_t cap, size_t* n_groups);
+
 /* Lookup-and-RESET (no reference analogue; building block of the multi-GPU local combiner, the counterpart of
  * the reference folding its per-CPU maps in user space, pkg/tracer/tracer.go:1159-1187): every flow that received
  * records since the previous drain is written to out_records (device memory, cap x 144 B) as a partial flow record

@@ -13,6 +13,8 @@ FA_MODE_ACCOUNTER, FA_MODE_KERNEL_MAP = 0, 1
 FA_F_ENABLE_RTT, FA_F_ENABLE_DNS, FA_F_ENABLE_SKETCH, FA_F_NO_FULL_CUT, FA_F_RINGBUF_FALLBACK, FA_F_ENABLE_PKT_DROP = 1, 2, 4, 8, 16, 32
 FA_F_NONBLOCKING_EVICT = 64
 FA_TOP_BYTES, FA_TOP_PACKETS, FA_TOP_MAX_K = 0, 1, 1 << 20
+FA_HIST_BYTES, FA_HIST_PACKETS, FA_HIST_DURATION, FA_HIST_RTT, FA_HIST_DNS_LATENCY = 0, 1, 2, 3, 4
+FA_HIST_MAX_BOUNDS = 63
 FA_GEN_UNIFORM, FA_GEN_ZIPF = 0, 1
 FA_ABI_VERSION = 1
 
@@ -66,6 +68,14 @@ GROUP_DTYPE = np.dtype([("key", "u1", 40), ("flows", "<u8"), ("bytes", "<u8"), (
 assert GROUP_DTYPE.itemsize == 88
 
 
+def hist_dtype(n_bounds):
+    """One row of fa_histogram_flows with n_bounds bounds: fa_hist_row, then n_bounds + 1 bucket counts
+    (FA_HIST_ROW_BYTES(n_bounds) bytes), include/flowagg.h."""
+    assert 1 <= n_bounds <= FA_HIST_MAX_BOUNDS, n_bounds
+    return np.dtype([("key", "u1", 40), ("flows", "<u8"), ("count", "<u8"), ("sum", "<u8"), ("min", "<u8"),
+                     ("max", "<u8"), ("counts", "<u8", (n_bounds + 1,))])
+
+
 class GenParams(C.Structure):
     _fields_ = [("seed", C.c_uint64), ("n_keys", C.c_uint64), ("dist", C.c_uint32), ("zipf_s_milli", C.c_uint32),
                 ("t0_ns", C.c_uint64), ("varying_desc", C.c_uint32), ("reserved", C.c_uint32)]
@@ -92,6 +102,8 @@ SIGNATURES = {
     "fa_expire_flows": (C.c_int, [C.c_void_p, C.c_uint64, C.c_uint64, C.c_uint64, C.POINTER(EvictOut), C.c_size_t,
                                   C.POINTER(C.c_size_t)]),
     "fa_group_flows": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_size_t, C.POINTER(C.c_size_t)]),
+    "fa_histogram_flows": (C.c_int, [C.c_void_p, C.c_void_p, C.c_uint32, C.c_void_p, C.c_uint32, C.c_void_p, C.c_size_t,
+                                     C.POINTER(C.c_size_t)]),
     "fa_evict": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_size_t,
                            C.POINTER(C.c_size_t)]),
     "fa_drain_active": (C.c_int, [C.c_void_p, C.c_void_p, C.c_size_t, C.POINTER(C.c_size_t)]),

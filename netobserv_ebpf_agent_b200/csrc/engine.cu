@@ -164,6 +164,9 @@ struct fa_engine {
     fa::GroupCtr* h_group_ctr = nullptr;      // pinned
     uint8_t* d_group_out = nullptr;           // ... and its staging of host-bound rows, group_out_cap rows
     uint64_t group_out_cap = 0;
+    uint32_t* d_hist_row_of = nullptr;        // fa_histogram_flows, under `mu`: row of each group, one u32 per group-table slot
+    uint8_t* d_hist_out = nullptr;            // ... and its staging of host-bound rows, hist_out_bytes
+    uint64_t hist_out_bytes = 0;
     uint32_t* d_slot_of = nullptr;            // per-sample slot scratch of the feature folds
     uint64_t feat_seq[3] = {0, 0, 0};         // running sample numbers (additional, dns, packet drops)
     uint32_t* d_route_tmp = nullptr; unsigned long long* d_route_counts = nullptr;
@@ -693,6 +696,7 @@ void fa_destroy(fa_engine* e) {
     if (e->h_expire_ctr) cudaFreeHost(e->h_expire_ctr);
     cudaFree(e->group.tab); cudaFree(e->group.list); cudaFree(e->group.ctr); cudaFree(e->d_group_out);
     if (e->h_group_ctr) cudaFreeHost(e->h_group_ctr);
+    cudaFree(e->d_hist_row_of); cudaFree(e->d_hist_out);
     cudaFree(e->sk.cms); cudaFree(e->sk.hll);
     cudaFree(e->dnsc.tab); cudaFree(e->dnsc_spare); cudaFree(e->dnsc.ctr); cudaFreeHost(e->h_dnsc_ctr);
     cudaFree(e->d_dnsc_state); cudaFree(e->d_dnsc_samples); cudaFree(e->d_dnsc_out); cudaFree(e->d_dnsc_warps);
@@ -1256,6 +1260,25 @@ static int grow_group_out(fa_engine* e, uint64_t n) {
     return FA_OK;
 }
 
+// The group table (all zero between calls), its list and counters for `live` flows, allocated on first use and grown
+// with the live count; with_row_of: also fa_histogram_flows' row index, one u32 per slot, grown with the table.
+static int grow_group_table(fa_engine* e, uint64_t live, bool with_row_of) {
+    uint64_t slots = 1024;                             // load factor <= 3/4: groups never outnumber the live flows
+    while (slots < (4 * live + 2) / 3) slots <<= 1;
+    if (!e->group.tab || e->group.mask + 1 < slots) {
+        cudaFree(e->group.tab); cudaFree(e->group.list); cudaFree(e->d_hist_row_of);
+        e->group.tab = nullptr; e->group.list = nullptr; e->group.mask = 0; e->d_hist_row_of = nullptr;
+        CU(cudaMalloc(&e->group.tab, slots * fa::kGroupSlotWords * 8));
+        CU(cudaMalloc(&e->group.list, slots * 4));
+        CU(cudaMemsetAsync(e->group.tab, 0, slots * fa::kGroupSlotWords * 8, e->stream));
+        e->group.mask = slots - 1;
+    }
+    if (with_row_of && !e->d_hist_row_of) CU(cudaMalloc(&e->d_hist_row_of, (e->group.mask + 1) * 4));
+    if (!e->group.ctr) CU(cudaMalloc(&e->group.ctr, sizeof(fa::GroupCtr)));
+    if (!e->h_group_ctr) CU(cudaHostAlloc(&e->h_group_ctr, sizeof(fa::GroupCtr), cudaHostAllocDefault));
+    return FA_OK;
+}
+
 int fa_group_flows(fa_engine* e, const uint8_t key_mask[40], fa_flow_group* out, size_t cap, size_t* n_groups) {
     if (n_groups) *n_groups = 0;
     if (!e || !key_mask || !n_groups || (!out && cap)) return fail(FA_E_INVAL, "fa_group_flows: null argument");
@@ -1271,18 +1294,7 @@ int fa_group_flows(fa_engine* e, const uint8_t key_mask[40], fa_flow_group* out,
     fa::GroupMask m;
     memcpy(m.w, key_mask, fa::kKeyBytes);
     m.w[4] &= 0x00FFFFFFFFFFFFFFull;                   // byte 39 (padding) is ignored
-    uint64_t slots = 1024;                             // load factor <= 3/4: groups never outnumber the live flows
-    while (slots < (4 * live + 2) / 3) slots <<= 1;
-    if (!e->group.tab || e->group.mask + 1 < slots) {
-        cudaFree(e->group.tab); cudaFree(e->group.list);
-        e->group.tab = nullptr; e->group.list = nullptr; e->group.mask = 0;
-        CU(cudaMalloc(&e->group.tab, slots * fa::kGroupSlotWords * 8));
-        CU(cudaMalloc(&e->group.list, slots * 4));
-        CU(cudaMemsetAsync(e->group.tab, 0, slots * fa::kGroupSlotWords * 8, st));
-        e->group.mask = slots - 1;
-    }
-    if (!e->group.ctr) CU(cudaMalloc(&e->group.ctr, sizeof(fa::GroupCtr)));
-    if (!e->h_group_ctr) CU(cudaHostAlloc(&e->h_group_ctr, sizeof(fa::GroupCtr), cudaHostAllocDefault));
+    if (int rc = grow_group_table(e, live, false)) return rc;
     const fa::GroupScratch s = e->group;
     CU(cudaMemsetAsync(s.ctr, 0, sizeof(fa::GroupCtr), st));
     uint64_t launched = fa::launch_group_scan(e->table, m, s, e->sm_count, st);
@@ -1311,6 +1323,101 @@ int fa_group_flows(fa_engine* e, const uint8_t key_mask[40], fa_flow_group* out,
     CU(cudaStreamSynchronize(st));
     e->st.kernel_launches += launched;
     e->st.d2h_bytes += d2h;
+    if (rc == FA_OK || rc == FA_E_2BIG) *n_groups = (size_t)n;
+    return rc;
+}
+
+// Per-group histograms of one per-flow value (evict.cu: launch_hist_*), on the groups of fa_group_flows: the group scan
+// builds the groups and their flow counts, the host reads their count (the one wait), then the rows are zeroed (device
+// `out` in place, host `out` through the histogram staging), indexed by group, binned by a second scan of the live flows
+// and completed from the group table, which is zeroed after (FA_E_2BIG: only zeroed).  Nothing of the flow table or the
+// counters is written.
+static_assert(FA_HIST_BYTES == fa::kHistBytes && FA_HIST_PACKETS == fa::kHistPackets && FA_HIST_DURATION == fa::kHistDuration &&
+              FA_HIST_RTT == fa::kHistRtt && FA_HIST_DNS_LATENCY == fa::kHistDnsLatency, "FA_HIST_* values");
+static_assert(FA_HIST_MAX_BOUNDS == fa::kHistMaxBounds && sizeof(fa_hist_row) == fa::kHistHeadWords * 8 &&
+              FA_HIST_ROW_BYTES(0) == fa::kHistHeadWords * 8 + 8 && offsetof(fa_hist_row, max) == 72, "fa_hist_row ABI");
+
+int fa_histogram_flows(fa_engine* e, const uint8_t key_mask[40], uint32_t value, const uint64_t* bounds, uint32_t n_bounds,
+                       void* out, size_t cap, size_t* n_groups) {
+    if (n_groups) *n_groups = 0;
+    if (!e || !key_mask || !bounds || !n_groups || (!out && cap)) return fail(FA_E_INVAL, "fa_histogram_flows: null argument");
+    if (value > FA_HIST_DNS_LATENCY) return fail(FA_E_INVAL, "fa_histogram_flows: unknown value %u", value);
+    if (n_bounds == 0 || n_bounds > FA_HIST_MAX_BOUNDS)
+        return fail(FA_E_INVAL, "fa_histogram_flows: n_bounds %u not in [1, %u]", n_bounds, FA_HIST_MAX_BOUNDS);
+    for (uint32_t i = 1; i < n_bounds; i++)
+        if (bounds[i] <= bounds[i - 1]) return fail(FA_E_INVAL, "fa_histogram_flows: bounds not strictly increasing at %u", i);
+    if (value == FA_HIST_RTT && !(e->cfg.flags & FA_F_ENABLE_RTT))
+        return fail(FA_E_INVAL, "fa_histogram_flows: FA_HIST_RTT needs an engine created with FA_F_ENABLE_RTT");
+    if (value == FA_HIST_DNS_LATENCY && !(e->cfg.flags & FA_F_ENABLE_DNS))
+        return fail(FA_E_INVAL, "fa_histogram_flows: FA_HIST_DNS_LATENCY needs an engine created with FA_F_ENABLE_DNS");
+    std::lock_guard<std::mutex> lk(e->mu);
+    CU(cudaSetDevice(e->device));
+    const bool out_dev = out && classify(out) == PTR_DEVICE;
+    if (out_dev && (reinterpret_cast<uintptr_t>(out) & 7))
+        return fail(FA_E_INVAL, "fa_histogram_flows: device out must be 8-byte aligned");
+    if (int rc = sync_counters(e)) return rc;          // the queued folds finish; exact live count
+    const uint64_t live = e->live_known;
+    if (live == 0) return FA_OK;
+    cudaStream_t st = e->stream;
+    fa::GroupMask m;
+    memcpy(m.w, key_mask, fa::kKeyBytes);
+    m.w[4] &= 0x00FFFFFFFFFFFFFFull;                   // byte 39 (padding) is ignored
+    fa::HistParams h{};
+    memcpy(h.bounds, bounds, n_bounds * sizeof(uint64_t));
+    h.n_bounds = n_bounds;
+    h.value = value;
+    const uint64_t row_bytes = FA_HIST_ROW_BYTES(n_bounds);
+    if (int rc = grow_group_table(e, live, true)) return rc;
+    const fa::GroupScratch s = e->group;
+    CU(cudaMemsetAsync(s.ctr, 0, sizeof(fa::GroupCtr), st));
+    uint64_t launched = fa::launch_group_scan(e->table, m, s, e->sm_count, st);
+    CU(cudaGetLastError());
+    CU(cudaMemcpyAsync(e->h_group_ctr, s.ctr, sizeof(fa::GroupCtr), cudaMemcpyDeviceToHost, st));
+    CU(cudaStreamSynchronize(st));
+    const uint64_t n = e->h_group_ctr->n;
+    int rc = FA_OK;
+    if (e->h_group_ctr->lost || n > live)
+        rc = fail(FA_E_CUDA, "fa_histogram_flows: %llu groups of %llu live flows, %llu folds without a slot", (unsigned long long)n,
+                  (unsigned long long)live, e->h_group_ctr->lost);
+    else if (n > cap)
+        rc = fail(FA_E_2BIG, "fa_histogram_flows: capacity %zu < %llu groups", cap, (unsigned long long)n);
+    uint64_t* rows = nullptr;
+    if (rc == FA_OK) {
+        if (out_dev) {
+            rows = reinterpret_cast<uint64_t*>(out);
+        } else if (e->hist_out_bytes < n * row_bytes) {
+            cudaFree(e->d_hist_out); e->d_hist_out = nullptr; e->hist_out_bytes = 0;
+            const uint64_t want = std::max<uint64_t>(n, std::min<uint64_t>(e->slots, 2 * n)) * row_bytes;
+            if (cudaMalloc(&e->d_hist_out, want) == cudaSuccess) {
+                e->hist_out_bytes = want;
+            } else {                                   // the group table is still cleared below
+                (void)cudaGetLastError();
+                e->d_hist_out = nullptr;
+                rc = fail(FA_E_CUDA, "fa_histogram_flows: no device memory for %llu B of staging", (unsigned long long)want);
+            }
+        }
+        if (rc == FA_OK && !rows) rows = reinterpret_cast<uint64_t*>(e->d_hist_out);
+    }
+    if (rows) {
+        CU(cudaMemsetAsync(rows, 0, n * row_bytes, st));
+        launched += fa::launch_hist_index(s, n, e->d_hist_row_of, e->sm_count, st);
+        launched += fa::launch_hist_scan(e->table, m, s, e->d_hist_row_of, h, rows, e->sm_count, st);
+        launched += fa::launch_hist_emit(s, n, n_bounds, rows, e->sm_count, st);
+        CU(cudaGetLastError());
+        CU(cudaMemcpyAsync(e->h_group_ctr, s.ctr, sizeof(fa::GroupCtr), cudaMemcpyDeviceToHost, st));
+    }
+    launched += fa::launch_group_emit(s, std::min<uint64_t>(n, s.mask + 1), nullptr, e->sm_count, st);   // clear the groups
+    CU(cudaGetLastError());
+    uint64_t d2h = 0;
+    if (rows && !out_dev) {
+        CU(cudaMemcpyAsync(out, rows, n * row_bytes, cudaMemcpyDeviceToHost, st));
+        d2h = n * row_bytes;
+    }
+    CU(cudaStreamSynchronize(st));
+    e->st.kernel_launches += launched;
+    e->st.d2h_bytes += d2h;
+    if (rows && e->h_group_ctr->lost)
+        rc = fail(FA_E_CUDA, "fa_histogram_flows: %llu flows did not find their group", e->h_group_ctr->lost);
     if (rc == FA_OK || rc == FA_E_2BIG) *n_groups = (size_t)n;
     return rc;
 }

@@ -779,4 +779,155 @@ int launch_group_emit(const GroupScratch& s, uint64_t n, uint64_t* out, int sm_c
     return 1;
 }
 
+// ---- fa_histogram_flows: per-group histograms of one per-flow value, without removing or changing anything ----------
+// Runs on the group table that launch_group_scan built (groups and flow counts).  Index: row_of[slot of group i] = i.
+// Scan (bitmap-driven, like group_scan_kernel): each live flow with the value finds its group by a read-only walk (it
+// exists: the group scan created it), picks its bucket and lands in row row_of[group].  The lanes of a warp take one
+// flow each per round; the lanes with equal (row, bucket) form a peer set and one leader per set folds the set into the
+// row.  Emit: one thread per row copies key and flows from the group slot and turns ~min into min.
+//
+// Row (u64 words, device `out` or staging, zeroed before the scan): [0, 5) key, [5] flows, [6] count (add), [7] sum (add),
+// [8] ~min (max), [9] max (max), [10 + b] bucket b (add).  Every accumulator has identity 0, so the rows do not depend on
+// the order of the updates.
+constexpr uint64_t kHistNoGroup = ~0ull;
+
+// The value of the row fa_evict_ex would return for `slot` now; false when that row has none (the decoder's presence
+// rules: duration needs a start, RTT a non-zero flow_rtt, DNS latency a DNS block with a non-zero id).
+__device__ __forceinline__ bool hist_value(const Table& t, uint64_t slot, uint32_t which, uint64_t& v) {
+    if (which == kHistBytes || which == kHistPackets) {
+        if (t.met) {
+            const uint8_t* M = t.met + slot * kMetLineBytes;
+            v = which == kHistBytes ? km_ld64(M + KM_BYTES) : km_ld32(M + KM_PACKETS);
+        } else {
+            const uint64_t* H = reinterpret_cast<const uint64_t*>(t.hot + slot * 2);
+            v = which == kHistBytes ? H[0] : (uint32_t)H[3];
+        }
+        return true;
+    }
+    if (which == kHistDuration) {
+        uint64_t s, e;
+        row_times(t, slot, s, e);
+        v = e >= s ? e - s : 0ull;
+        return s != 0;
+    }
+    if (which == kHistRtt) {
+        const uint64_t* S = reinterpret_cast<const uint64_t*>(t.feat_add + slot * kAddState);
+        v = S[0] ? S[1] : 0ull;                                      // additional.flow_rtt: the max of the samples
+        return v != 0;
+    }
+    const uint64_t* S = reinterpret_cast<const uint64_t*>(t.feat_dns + slot * kDnsState);
+    v = S[1];                                                        // dns.latency: the max; dns.id: last non-zero id
+    return S[0] != 0 && (S[2] & 0xFFFFull) != 0;
+}
+
+// The group-table slot of masked key k: linear probing from its slot hash up to the first EMPTY slot, every slot at
+// most once.  Nothing is written.
+__device__ __forceinline__ uint64_t hist_group(const GroupScratch& s, const uint64_t k[5]) {
+    uint64_t slot = slot_hash(key_premix(k[0], k[1], k[2], k[3], k[4])) & s.mask;
+    for (uint64_t probes = 0; probes <= s.mask; probes++, slot = (slot + 1) & s.mask) {
+        const unsigned long long* G = s.tab + slot * kGroupSlotWords;
+        if (G[5] == 0ull) break;
+        unsigned long long diff = 0;
+#pragma unroll
+        for (int w = 0; w < 5; w++) diff |= G[w] ^ k[w];
+        if (diff == 0) return slot;
+    }
+    return kHistNoGroup;
+}
+
+__global__ void __launch_bounds__(256) hist_index_kernel(GroupScratch s, unsigned long long n, uint32_t* __restrict__ row_of) {
+    for (unsigned long long i = blockIdx.x * (unsigned long long)blockDim.x + threadIdx.x; i < n; i += (unsigned long long)gridDim.x * blockDim.x)
+        row_of[s.list[i]] = (uint32_t)i;
+}
+
+__global__ void __launch_bounds__(256) hist_scan_kernel(Table t, GroupMask m, GroupScratch s, const uint32_t* __restrict__ row_of,
+                                                        HistParams h, unsigned long long* __restrict__ rows) {
+    FA_DYN_SMEM(smem);
+    unsigned long long* bounds = reinterpret_cast<unsigned long long*>(smem);       // the search reads shared memory
+    for (uint32_t i = threadIdx.x; i < h.n_bounds; i += blockDim.x) bounds[i] = h.bounds[i];
+    __syncthreads();
+    const int lane = threadIdx.x & 31;
+    const uint64_t row_words = kHistHeadWords + h.n_bounds + 1;
+    TOP_FOR_WORDS(t, w) {
+        uint32_t r = t.occ[w];
+        while (__any_sync(0xFFFFFFFFu, r != 0u)) {             // converged rounds: at most one flow per lane
+            bool have = false;
+            uint32_t row = 0, b = 0;
+            uint64_t v = 0;
+            if (r != 0u) {
+                const uint64_t slot = w * 32 + (__ffs(r) - 1);
+                r &= r - 1;
+                if (hist_value(t, slot, h.value, v)) {
+                    const uint64_t* L = reinterpret_cast<const uint64_t*>(t.ident) + slot * (kIdentBytes / 8);
+                    uint64_t k[5];
+#pragma unroll
+                    for (int i = 0; i < 5; i++) k[i] = L[i] & m.w[i];
+                    const uint64_t g = hist_group(s, k);
+                    if (g == kHistNoGroup) {
+                        atomicAdd(&s.ctr->lost, 1ull);
+                    } else {
+                        have = true;
+                        row = row_of[g];
+                        // the number of bounds below v: bucket b holds bounds[b-1] < v <= bounds[b] (b = n_bounds: +Inf)
+#pragma unroll
+                        for (uint32_t step = 32; step > 0; step >>= 1)
+                            if (b + step <= h.n_bounds && bounds[b + step - 1] < v) b += step;
+                    }
+                }
+            }
+            uint32_t peers = __ballot_sync(0xFFFFFFFFu, have) & __match_any_sync(0xFFFFFFFFu, row) & __match_any_sync(0xFFFFFFFFu, b);
+            if (!have) peers = 0u;
+            const int np = __popc(peers);
+            // step q: every lane reads the q-th lane of its own set (the leader is lane 0 of it)
+            uint64_t sum = v, mx = v, nmin = ~v;
+            const int most = (int)__reduce_max_sync(0xFFFFFFFFu, (unsigned)np);
+            for (int q = 1; q < most; q++) {
+                const int src = q < np ? (int)__fns(peers, 0, q + 1) : lane;
+                const uint64_t x = __shfl_sync(0xFFFFFFFFu, v, src);
+                if (q < np) { sum += x; mx = x > mx ? x : mx; nmin = ~x > nmin ? ~x : nmin; }
+            }
+            if (have && lane == __ffs(peers) - 1) {
+                unsigned long long* R = rows + (uint64_t)row * row_words;
+                red_add_u64(R + 6, (unsigned long long)np);
+                if (sum) red_add_u64(R + 7, sum);
+                if (nmin) red_max_u64(R + 8, nmin);
+                if (mx) red_max_u64(R + 9, mx);
+                red_add_u64(R + kHistHeadWords + b, (unsigned long long)np);
+            }
+        }
+    }
+}
+
+__global__ void __launch_bounds__(256) hist_emit_kernel(GroupScratch s, unsigned long long n, uint32_t n_bounds, unsigned long long* __restrict__ rows) {
+    for (unsigned long long i = blockIdx.x * (unsigned long long)blockDim.x + threadIdx.x; i < n; i += (unsigned long long)gridDim.x * blockDim.x) {
+        const unsigned long long* G = s.tab + (uint64_t)s.list[i] * kGroupSlotWords;
+        unsigned long long* R = rows + i * (kHistHeadWords + n_bounds + 1);
+        for (int w = 0; w < 5; w++) R[w] = G[w];
+        R[5] = G[6];                                            // flows
+        R[8] = R[6] ? ~R[8] : 0ull;                             // min: 0 when no flow of the group has the value
+    }
+}
+
+int launch_hist_index(const GroupScratch& s, uint64_t n, uint32_t* row_of, int sm_count, cudaStream_t st) {
+    if (!n) return 0;
+    const uint64_t cap = (uint64_t)sm_count * 8, per_row = (n + 255) / 256;
+    FA_LAUNCH(hist_index_kernel, (int)(per_row < cap ? per_row : cap), 256, 0, st, s, (unsigned long long)n, row_of);
+    return 1;
+}
+
+int launch_hist_scan(const Table& t, const GroupMask& m, const GroupScratch& s, const uint32_t* row_of, const HistParams& h,
+                     uint64_t* rows, int sm_count, cudaStream_t st) {
+    FA_LAUNCH(hist_scan_kernel, sm_count * 8, 256, kHistMaxBounds * 8, st, t, m, s, row_of, h,
+              reinterpret_cast<unsigned long long*>(rows));
+    return 1;
+}
+
+int launch_hist_emit(const GroupScratch& s, uint64_t n, uint32_t n_bounds, uint64_t* rows, int sm_count, cudaStream_t st) {
+    if (!n) return 0;
+    const uint64_t cap = (uint64_t)sm_count * 8, per_row = (n + 255) / 256;
+    FA_LAUNCH(hist_emit_kernel, (int)(per_row < cap ? per_row : cap), 256, 0, st, s, (unsigned long long)n, n_bounds,
+              reinterpret_cast<unsigned long long*>(rows));
+    return 1;
+}
+
 }  // namespace fa

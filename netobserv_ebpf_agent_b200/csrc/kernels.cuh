@@ -167,6 +167,23 @@ int launch_group_scan(const Table& t, const GroupMask& m, const GroupScratch& s,
 // their slots, so that the table is all zero again.
 int launch_group_emit(const GroupScratch& s, uint64_t n, uint64_t* out, int sm_count, cudaStream_t st);
 
+// fa_histogram_flows (evict.cu): on the group table of launch_group_scan, a per-group histogram of one per-flow value.
+// Row (fa_hist_row): kHistHeadWords u64 of header, then n_bounds + 1 u64 bucket counts.
+enum : uint32_t { kHistBytes = 0, kHistPackets = 1, kHistDuration = 2, kHistRtt = 3, kHistDnsLatency = 4 };   // FA_HIST_*
+constexpr int kHistMaxBounds = 63;
+constexpr int kHistHeadWords = 10;                 // key (5), flows, count, sum, min, max
+// Kernel argument (512 B of parameter space): the value and the Prometheus `le` bounds, strictly increasing.
+struct HistParams { unsigned long long bounds[kHistMaxBounds]; uint32_t n_bounds, value; };
+// row_of[list[i]] = i for the n listed groups (row_of: one u32 per group-table slot).
+int launch_hist_index(const GroupScratch& s, uint64_t n, uint32_t* row_of, int sm_count, cudaStream_t st);
+// Bin every live flow of `t` that has the value into row row_of[its group] of `rows` (device, all zero before; n rows
+// of kHistHeadWords + n_bounds + 1 u64).  Reads `t` and the group table only.
+int launch_hist_scan(const Table& t, const GroupMask& m, const GroupScratch& s, const uint32_t* row_of, const HistParams& h,
+                     uint64_t* rows, int sm_count, cudaStream_t st);
+// Fill row i's key and flows from the i-th listed group and turn its ~min into min.  The group table is left as it is
+// (launch_group_emit with out == nullptr clears it).
+int launch_hist_emit(const GroupScratch& s, uint64_t n, uint32_t n_bounds, uint64_t* rows, int sm_count, cudaStream_t st);
+
 // sketches
 int launch_cms_query(const SketchParams& sk, const uint4* keys, uint32_t n, unsigned long long* est, cudaStream_t st);
 int launch_hll_pack(const SketchParams& sk, uint8_t* out_regs, cudaStream_t st);

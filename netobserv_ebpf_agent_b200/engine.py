@@ -258,6 +258,23 @@ class FlowAggEngine:
         check(lib().fa_group_flows(self._h, m.ctypes.data, out.ctypes.data, cap, C.byref(got)))
         return out[: got.value]
 
+    def histogram_flows(self, mask, value, bounds, cap=None):
+        """Per-group histograms of one per-flow value (FA_HIST_*) over the live flows, grouped by a 40-byte key mask
+        (group_mask), without changing anything -> a hist_dtype(len(bounds)) array, one row per group, in unspecified
+        order.  bounds: the Prometheus `le` upper bounds, strictly increasing (counts are per bucket, the last bucket is
+        +Inf).  cap: room in groups (default: the live count right now)."""
+        from ._lib import FA_HIST_MAX_BOUNDS, hist_dtype
+        m = np.ascontiguousarray(mask, dtype=np.uint8).reshape(-1)
+        assert m.size == 40, m.size
+        b = np.ascontiguousarray(bounds, dtype=np.uint64).reshape(-1)
+        if cap is None:
+            cap = max(self.live_flows(), 1)
+        out = np.zeros(cap, hist_dtype(min(max(b.size, 1), FA_HIST_MAX_BOUNDS)))     # other sizes: FA_E_INVAL below
+        got = C.c_size_t(0)
+        check(lib().fa_histogram_flows(self._h, m.ctypes.data, value, b.ctypes.data, b.size, out.ctypes.data, cap,
+                                       C.byref(got)))
+        return out[: got.value]
+
     def read_spilled(self, cap=131072):
         """KERNEL_MAP mode with FA_F_RINGBUF_FALLBACK: the single-packet records that could not enter the full map
         (the batched equivalent of reading the direct_flows ring buffer) -> (n,144) uint8 array."""
