@@ -25,6 +25,11 @@
 //      when they can change it).
 // The cache is flushed with the same reductions when the CTA runs out of tiles.
 //
+// The cache: 96 entries as 12 sets x 8 ways, the set picked by the upper half of the 32-bit slot hash.  A set's eight
+// 16-bit tags (lower hash bits | 1) are one 16-byte word, so a lookup is one shared-memory load and eight compares
+// before it touches an entry; only a way whose tag matches is checked by its full hash and then by the 114 bytes.  A
+// flow with two records in one tile takes a free way of its set, first come first served, and keeps it for the launch.
+//
 // Exactness of the order-dependent fields (eth_protocol / dscp / sampling = last non-zero,
 // MACs = first non-zero, everything else = first record; flow_content.go:45-59,
 // account.go:95): while every record of a flow carries the same 74-byte descriptor the
@@ -43,8 +48,9 @@ constexpr int kTeams     = 1024 / kTile;        // teams per CTA (one CTA per SM
                                                 // bubbles (tile wait, team barriers); 8 x 128 stays selectable (FA_K1_TILE=128)
 constexpr int kCtaThreads = kTile * kTeams;
 constexpr int kRepSlots  = 2 * kTile;
-constexpr int kHot2 = 32;                       // second-chance entries (another slice of the hash)
-constexpr int kHotEntries = 64 + kHot2;         // 64 primary entries + the second-chance ones
+constexpr int kHotWays = 8;                     // ways of a cache set: their 16-bit tags are one 16-byte shared-memory load
+constexpr int kHotSets = 12;
+constexpr int kHotEntries = kHotSets * kHotWays;
 typedef uint8_t RepIdx;                         // index of a record inside its tile
 static_assert(kTile == 128 || kTile == 256, "election slots and lists keep the tile index in 8 bits; 1024 threads per CTA");
 #ifndef FA_K1_STREAM_HINT
@@ -83,13 +89,29 @@ struct __align__(16) HotEntry {                   // 208 B: a stride of 52 words
 };
 static_assert(sizeof(HotEntry) == 208, "HotEntry stride");
 static_assert(kTile != 128 || sizeof(TeamSmem) == 26496, "TeamSmem has no padding to spare");
-struct __align__(128) AggSmem {                   // 232,080 B of the 232,448 B (227 KB) an sm_90 CTA may use
+struct __align__(128) AggSmem {                   // 232,272 B of the 232,448 B (227 KB) an sm_90 CTA may use
     TeamSmem team[kTeams];
     HotEntry hot[kHotEntries];
+    alignas(16) uint16_t hot_tag[kHotEntries];    // per entry: low 16 hash bits | 1 of the live entry, 0 = none (written after state = 2)
     TeamCtl  ctl[kTeams];
     uint32_t n_insert, n_spill, any_dirty, pad;
 };
 static_assert(sizeof(AggSmem) <= 232448, "K1 shared memory exceeds what one sm_90 CTA can opt into");
+
+// Cache set and tag of a flow, from the low 32 bits of its slot hash; the ways of `tags` (8 x 16 bit) that hold `tag`.
+__device__ __forceinline__ uint32_t hot_set(uint32_t h) { return ((h >> 16) * (uint32_t)kHotSets) >> 16; }
+__device__ __forceinline__ uint32_t hot_tag_of(uint32_t h) { return (h & 0xFFFFu) | 1u; }
+__device__ __forceinline__ uint32_t hot_ways_with(uint4 tags, uint32_t tag) {
+    const uint32_t w[4] = {tags.x, tags.y, tags.z, tags.w};
+    uint32_t m = 0;
+#pragma unroll
+    for (int i = 0; i < 4; i++) {
+        const uint32_t x = w[i] ^ (tag * 0x10001u);
+        m |= ((x & 0xFFFFu) == 0u ? 1u : 0u) << (2 * i) | ((x >> 16) == 0u ? 2u : 0u) << (2 * i);
+    }
+    return m;
+}
+static_assert(kHotWays * sizeof(uint16_t) == sizeof(uint4), "a set's tags are read as one uint4");
 
 __device__ __forceinline__ void team_sync(int team) { named_barrier_sync(team + 1, kTile); }
 
@@ -235,7 +257,7 @@ aggregate_kernel(const uint4* __restrict__ recs, uint32_t n, Table t, uint64_t e
     const bool use_cache = (opt & 2u) == 0;
 
     if (threadIdx.x == 0) { cs.n_insert = 0; cs.n_spill = 0; cs.any_dirty = 0; }
-    if (threadIdx.x < kHotEntries) cs.hot[threadIdx.x].state = 0;
+    if (threadIdx.x < kHotEntries) { cs.hot[threadIdx.x].state = 0; cs.hot_tag[threadIdx.x] = 0; }
     if (tid == 0) {
         mbar_init(&tc.full_bar, 1);
         fence_barrier_init();
@@ -279,11 +301,14 @@ aggregate_kernel(const uint4* __restrict__ recs, uint32_t n, Table t, uint64_t e
                                                         u64_of(r1.z, r1.w), u64_of(r2.x, r2.y)));
                 s.hs[tid] = (uint32_t)h;
                 // ---- hot-flow cache: an exact 114-byte match folds the record on-chip, no table traffic
-                uint32_t cidx = (uint32_t)h >> 26;                        // primary way
-                if (!(*reinterpret_cast<volatile uint32_t*>(&cs.hot[cidx].state) == 2u && cs.hot[cidx].hash == (uint32_t)h))
-                    cidx = 64u + (((uint32_t)h >> 21) & (uint32_t)(kHot2 - 1));              // second chance
-                HotEntry& ce = cs.hot[cidx];
-                if (use_cache && *reinterpret_cast<volatile uint32_t*>(&ce.state) == 2u && ce.hash == (uint32_t)h) {
+                const uint32_t cset = hot_set((uint32_t)h);
+                uint32_t cidx = kHotEntries;                              // the way of the set that holds this hash, if any
+                for (uint32_t m = hot_ways_with(*reinterpret_cast<const uint4*>(&cs.hot_tag[cset * kHotWays]), hot_tag_of((uint32_t)h)); m; m &= m - 1u) {
+                    const uint32_t i = cset * kHotWays + (uint32_t)__ffs((int)m) - 1u;
+                    if (*reinterpret_cast<volatile uint32_t*>(&cs.hot[i].state) == 2u && cs.hot[i].hash == (uint32_t)h) { cidx = i; break; }
+                }
+                if (use_cache && cidx < (uint32_t)kHotEntries) {
+                    HotEntry& ce = cs.hot[cidx];
                     const uint4 r3 = R[3], r4 = R[4];
                     bool same = eq4_masked(ce.line[0], r0, chunk_mask(0)) && eq4_masked(ce.line[1], r1, chunk_mask(1)) &&
                                 eq4_masked(ce.line[2], r2, chunk_mask(2)) && eq4_masked(ce.line[3], r4, chunk_mask(3));
@@ -515,13 +540,22 @@ aggregate_kernel(const uint4* __restrict__ recs, uint32_t n, Table t, uint64_t e
                 const uint32_t t_flags = a0.w & 0xFFFFu, n_dups = kSketch ? (a0.w >> 16) & 0xFFu : a0.w >> 16;
                 const uint64_t t_ns = u64_of(a1.x, a1.z), t_end = u64_of(a1.y, a1.w);
                 const uint64_t v_ns = t_ns, v_end = t_end;           // the cache entry's windows: high words only
-                // a flow that shows up several times in one tile is hot: give it a cache entry if one is free
+                // a flow that shows up several times in one tile is hot: give it a way of its set if one is free and it
+                // has none yet (an entry another team is filling right now is not seen: the flow then holds two ways,
+                // which costs a way and nothing else, every live entry is flushed)
                 if (use_cache && n_dups >= kHotMinDups && my_slot != kResSpill) {
-                    const uint32_t hh = s.hs[my_ridx];
-                    uint32_t iidx = hh >> 26;
-                    if (*reinterpret_cast<volatile uint32_t*>(&cs.hot[iidx].state) != 0u && cs.hot[iidx].hash != hh) iidx = 64u + ((hh >> 21) & (uint32_t)(kHot2 - 1));
-                    HotEntry& ce = cs.hot[iidx];
-                    if (*reinterpret_cast<volatile uint32_t*>(&ce.state) == 0u && atomicCAS(&ce.state, 0u, 1u) == 0u) {
+                    const uint32_t hh = s.hs[my_ridx], iset = hot_set(hh);
+                    const uint4 tags = *reinterpret_cast<const uint4*>(&cs.hot_tag[iset * kHotWays]);
+                    bool cached = false;
+                    for (uint32_t m = hot_ways_with(tags, hot_tag_of(hh)); m; m &= m - 1u)
+                        cached = cached || cs.hot[iset * kHotWays + (uint32_t)__ffs((int)m) - 1u].hash == hh;
+                    uint32_t iidx = kHotEntries;
+                    for (uint32_t m = cached ? 0u : hot_ways_with(tags, 0u); m; m &= m - 1u) {
+                        const uint32_t i = iset * kHotWays + (uint32_t)__ffs((int)m) - 1u;
+                        if (atomicCAS(&cs.hot[i].state, 0u, 1u) == 0u) { iidx = i; break; }
+                    }
+                    if (iidx < (uint32_t)kHotEntries) {
+                        HotEntry& ce = cs.hot[iidx];
 #pragma unroll
                         for (int c = 0; c < 8; c++) ce.line[c] = ld_cg_u4(&t.ident[(size_t)my_slot * 8 + c]);
                         *reinterpret_cast<uint4*>(&ce.acc[0]) = make_uint4(0, 0, 0, 0);
@@ -530,6 +564,8 @@ aggregate_kernel(const uint4* __restrict__ recs, uint32_t n, Table t, uint64_t e
                         ce.ns_hi = (uint32_t)(v_ns >> 32); ce.end_hi = (uint32_t)(v_end >> 32);
                         __threadfence_block();
                         *reinterpret_cast<volatile uint32_t*>(&ce.state) = 2u;
+                        __threadfence_block();
+                        *reinterpret_cast<volatile uint16_t*>(&cs.hot_tag[iidx]) = (uint16_t)hot_tag_of(hh);
                         if (kProf) c_install++;
                     }
                 }

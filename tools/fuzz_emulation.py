@@ -2,7 +2,8 @@
 """Randomised parity runs of the kernels under the host emulation (no GPU): the K1 emulation against the oracle's Accounter
 (`k1`), the emulated C ABI with full cuts / chunking / re-fold (`engine`), and the feature folds + K7 through it (`features`).
 Test infrastructure, like tests/emul/: usage `python tools/fuzz_emulation.py k1|engine|features SEED SECONDS`.
-Round 2, shipped kernels: k1 366 iterations, engine 204, features 569 — no mismatch."""
+Round 2, shipped kernels: k1 366 iterations, engine 204, features 569 — no mismatch.  With the 12 x 8 hot-flow cache:
+k1 50 iterations (seed 5, 150 s) — no mismatch."""
 import os
 import sys
 import time
