@@ -23,10 +23,9 @@
 
 namespace fa {
 
-constexpr uint32_t kDnsNone = 0xFFFFFFFFu;      // no entry (table full) / "no index"
+constexpr uint32_t kDnsNone = 0xFFFFFFFFu;      // no entry (every slot holds another key) / "no index"
 constexpr uint32_t kDnsEmit = 0xFFFFFFFEu;      // retired, produced a sample
 constexpr uint32_t kDnsSkip = 0xFFFFFFFDu;      // retired, no sample
-constexpr uint32_t kDnsProbeLimit = 4096;
 constexpr uint32_t kDnsQR = 0x8000u;            // DNS_QR_FLAG (dns_tracker.h:10)
 
 struct DnsPkt {                                 // one parsed 104-byte DNS packet record
@@ -55,10 +54,13 @@ __device__ __forceinline__ DnsPkt dns_parse(const uint8_t* P) {
     return p;
 }
 
-// find the key's entry, creating an absent one when the key is new; kDnsNone when the probe sequence is exhausted
+// find the key's entry, creating an absent one when the key is new.  The walk may pass every slot of the table: a run
+// of occupied slots is not bounded by the pending queries (every packet's key takes an entry until the next rebuild, and
+// keys can be chosen to share a home slot), only by the table's fill, which fa_ingest_dns_packets keeps at one half.
+// So the walk ends at the key or at an empty slot; kDnsNone (every slot holds another key) cannot happen in such a table.
 __device__ uint32_t dns_find_or_create(const DnsCorr& d, const uint64_t k[5]) {
     uint64_t slot = slot_hash(key_premix(k[0], k[1], k[2], k[3], k[4])) & d.mask;
-    for (uint32_t probes = 0; probes < kDnsProbeLimit; ) {
+    for (uint64_t probes = 0; probes <= d.mask; ) {
         DnsEntry* E = &d.tab[slot];
         const uint32_t tag = *reinterpret_cast<volatile uint32_t*>(&E->tag);
         if (tag == 0u) {
@@ -86,7 +88,8 @@ __device__ uint32_t dns_find_or_create(const DnsCorr& d, const uint64_t k[5]) {
 }
 
 // The reference's step for one packet whose turn it is (dns_tracker.h:92-110) + the sample of flows.c:291-330.
-// `E` may be null: the key has no entry and none could be made (table exhausted).  Returns true when a sample was written.
+// `E` may be null: the key has no entry and none could be made (a table with no empty slot, which the engine's fill rule
+// rules out; the query is then reported as -E2BIG).  Returns true when a sample was written.
 __device__ bool dns_step(const DnsCorr& d, DnsEntry* E, const DnsPkt& p, const uint8_t* P, uint8_t* S) {
     int dns_errno = 0;
     uint64_t latency = 0;
@@ -239,6 +242,7 @@ __global__ void dns_rebuild_kernel(DnsCorr from, DnsCorr to) {
         for (int c = 0; c < 5; c++) k[c] = E->key[c];
         const uint32_t slot = dns_find_or_create(to, k);            // counts into to.ctr[DNSC_CREATED] (the same counters)
         if (slot != kDnsNone) { to.tab[slot].ts = E->ts; to.tab[slot].present = 1u; }
+        else atomicAdd(&to.ctr[DNSC_PRESENT], ~0ull);               // not re-placed (cannot happen at half fill): the query is gone
     }
 }
 

@@ -1576,7 +1576,9 @@ int fa_ingest_dns_packets(fa_engine* e, const void* pkts, size_t n) {
     CU(cudaSetDevice(e->device));
     if (int rc = dnsc_init(e)) return rc;
     // a chunk never takes more than a quarter of the table: with at most max_entries = slots / 4 present keys after a
-    // rebuild the table stays at most half full, so a probe sequence cannot run out
+    // rebuild the table stays at most half full.  That bounds the fill, not the length of a run: every packet takes an
+    // entry, and keys can share a home slot, so one run can hold every entry in use.  The walk of dns_find_or_create is
+    // therefore bounded by the table size, and always ends at the key or at an empty slot.
     const uint64_t cmax = std::min<uint64_t>(e->dnsc_chunk, e->dnsc_slots / 4);
     Input in(e, pkts, n, fa::kDnsRecBytes, cmax, std::min<uint64_t>(cmax, stage_records(e)), WINDOW_NONE);
     if (in.misaligned(8)) return fail(FA_E_INVAL, "%s: device packets must be 8-byte aligned", who);
