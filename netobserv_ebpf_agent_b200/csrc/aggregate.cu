@@ -2,9 +2,12 @@
 // open-addressed flow table with the semantics of the reference's userspace Accounter
 // (pkg/flow/account.go:82-96 + pkg/model/flow_content.go:28-61).
 //
-// One persistent CTA per SM, 1024 threads = 4 teams of 256 (FA_K1_TILE).  Each team owns a stream
-// of 256-record tiles and synchronises with a named barrier; all teams share a small cache of
-// the hottest flows.  Per tile:
+// One persistent CTA per SM, 1024 threads = 4 teams of 256 (FA_K1_TILE).  Each team works through
+// 256-record tiles and synchronises with a named barrier; all teams share a small cache of the
+// hottest flows.  A team's first tile is blockIdx.x * kTeams + team; it claims every later one from
+// a per-launch counter while it works on the current one, so teams that run ahead take the tail of
+// the batch instead of waiting on a fixed stride.  The last CTA out resets the counter and writes
+// the live-flow count into the host's mapped ring (no copy node between launches).  Per tile:
 //   TMA bulk copy (cp.async.bulk + mbarrier) stages 36 KB of records in shared memory
 //   -> E: each thread hashes one record; a record of a cached hot flow folds straight into
 //      the cache's shared-memory accumulators; every other record writes its own values into
@@ -23,7 +26,7 @@
 //   -> one lane per flow, from the accumulators alone: three fire-and-forget reductions on
 //      the 32-byte hot line (RED.add bytes, RED.add packets, RED.max end; start / flags only
 //      when they can change it).
-// The cache is flushed with the same reductions when the CTA runs out of tiles.
+// The cache is flushed with the same reductions when the CTA runs out of tiles: it lives for one launch.
 //
 // The cache: 96 entries as 12 sets x 8 ways, the set picked by the upper half of the 32-bit slot hash.  A set's eight
 // 16-bit tags (lower hash bits | 1) are one 16-byte word, so a lookup is one shared-memory load and eight compares
@@ -77,6 +80,8 @@ struct __align__(128) TeamSmem {                  // 26,496 B per team (128-reco
 struct __align__(16) TeamCtl {                    // kept outside TeamSmem so that the teams + the cache fit in 227 KB
     unsigned long long full_bar;                  // mbarrier of the team's tile
     uint32_t nrep, done;                          // representatives of the tile; warps that are through with its probes
+    uint32_t next[2];                             // the team's next tile, claimed during tile `it`, in next[it & 1]
+    uint32_t pad[2];
 };
 struct __align__(16) HotEntry {                   // 208 B: a stride of 52 words keeps 8 entries on distinct banks
     uint4    line[8];                             // copy of the flow's identity line
@@ -89,7 +94,7 @@ struct __align__(16) HotEntry {                   // 208 B: a stride of 52 words
 };
 static_assert(sizeof(HotEntry) == 208, "HotEntry stride");
 static_assert(kTile != 128 || sizeof(TeamSmem) == 26496, "TeamSmem has no padding to spare");
-struct __align__(128) AggSmem {                   // 232,272 B of the 232,448 B (227 KB) an sm_90 CTA may use
+struct __align__(128) AggSmem {                   // 232,320 B (sizeof) of the 232,448 B (227 KB) an sm_90 CTA may use
     TeamSmem team[kTeams];
     HotEntry hot[kHotEntries];
     alignas(16) uint16_t hot_tag[kHotEntries];    // per entry: low 16 hash bits | 1 of the live entry, 0 = none (written after state = 2)
@@ -114,6 +119,11 @@ __device__ __forceinline__ uint32_t hot_ways_with(uint4 tags, uint32_t tag) {
 static_assert(kHotWays * sizeof(uint16_t) == sizeof(uint4), "a set's tags are read as one uint4");
 
 __device__ __forceinline__ void team_sync(int team) { named_barrier_sync(team + 1, kTile); }
+
+// Per-launch words of K1 in Counters::scratch, zero between launches: [0] counts the tiles claimed after each team's
+// first, [2] is the ticket of CTAs that are through, whose last holder zeroes both.  ([1] is fixup_apply's ticket.)
+__device__ __forceinline__ unsigned int* k1_tile_claims(Counters* c) { return reinterpret_cast<unsigned int*>(&c->scratch[0]); }
+__device__ __forceinline__ unsigned int* k1_exit_ticket(Counters* c) { return reinterpret_cast<unsigned int*>(&c->scratch[2]); }
 
 __device__ __forceinline__ void issue_tile_load(TeamSmem& s, TeamCtl& tc, const uint4* recs, uint32_t n, uint32_t tile_idx) {
     const uint32_t first = tile_idx * kTile;
@@ -250,10 +260,12 @@ aggregate_kernel(const uint4* __restrict__ recs, uint32_t n, Table t, uint64_t e
     const int tid = threadIdx.x & (kTile - 1), lane = tid & 31, warp = tid >> 5;     // within the team
     TeamSmem& s = cs.team[team];
     TeamCtl& tc = cs.ctl[team];
-    if (kDevN) n = min(n, (uint32_t)ctr->launch_n);            // size known on the device only (multi-GPU receive side)
-    const uint32_t n_tiles = (n + kTile - 1) / kTile;
-    const uint32_t tile_stride = gridDim.x * kTeams;
+    // Tile schedule: every team starts on tile blockIdx.x * kTeams + team; each later tile is claimed from the launch's
+    // counter (gridDim.x * kTeams + the count of earlier claims), so a team that finishes early takes the next tile
+    // instead of the slowest teams' tails being fixed by a static stride.
     const uint32_t tile0 = blockIdx.x * kTeams + team;
+    const uint32_t claim_base = gridDim.x * kTeams;
+    unsigned int* const tile_claims = k1_tile_claims(ctr);
     const bool use_cache = (opt & 2u) == 0;
 
     if (threadIdx.x == 0) { cs.n_insert = 0; cs.n_spill = 0; cs.any_dirty = 0; }
@@ -267,6 +279,9 @@ aggregate_kernel(const uint4* __restrict__ recs, uint32_t n, Table t, uint64_t e
     *reinterpret_cast<uint4*>(&s.acc[tid][0]) = make_uint4(0, 0, 0, 0);
     *reinterpret_cast<uint4*>(&s.acc[tid][4]) = make_uint4(0, 0, 0, 0);
     s.tdirty[tid] = 0;
+    pdl_wait();                                                    // the kernels before this launch have completed
+    if (kDevN) n = min(n, (uint32_t)ctr->launch_n);            // size known on the device only (multi-GPU receive side)
+    const uint32_t n_tiles = (n + kTile - 1) / kTile;
     __syncthreads();
     if (tid == 0 && tile0 < n_tiles) issue_tile_load(s, tc, recs, n, tile0);
 
@@ -282,11 +297,15 @@ aggregate_kernel(const uint4* __restrict__ recs, uint32_t n, Table t, uint64_t e
     long long pt = kProf ? clock64() : 0;
     uint32_t c_cached = 0, c_reps = 0, c_slow = 0, c_install = 0, c_collide = 0, c_p1fast = 0, c_unsettled = 0;   // kProf only
 
-    for (uint32_t it = 0;; ++it) {
-        const uint32_t tile_idx = tile0 + it * tile_stride;
-        if (tile_idx >= n_tiles) break;
+    uint32_t tile_idx = tile0;
+    for (uint32_t it = 0; tile_idx < n_tiles; ++it) {               // `it` counts the team's own tiles: mbarrier parity
         const uint32_t first = tile_idx * kTile;
         const uint32_t cnt = min((uint32_t)kTile, n - first);
+        // claim the team's next tile now, so that the atomic's round trip overlaps this tile's E phase; it is published
+        // in next[it & 1] before S1 and read by the warp that re-arms the TMA (after S1) and by every thread after S2.
+        // The other word of the pair is still being read by threads that have not left the previous iteration.
+        uint32_t claimed = 0;
+        if (tid == 0) claimed = claim_base + atomicAdd(tile_claims, 1u);
         mbar_wait(&tc.full_bar, it & 1u);
         FA_PROF_MARK(0);                                           // waiting for the tile
 
@@ -400,6 +419,7 @@ aggregate_kernel(const uint4* __restrict__ recs, uint32_t n, Table t, uint64_t e
             lbase = __shfl_sync(0xFFFFFFFFu, lbase, 0);
             if (is_rep) s.glist[lbase + __popc(pending & lt_mask)] = (RepIdx)tid;
         }
+        if (tid == 0) tc.next[it & 1u] = claimed;
         FA_PROF_MARK(1);                                           // E phase
         team_sync(team);                                           // S1: folds, hashes and the list are complete
         FA_PROF_MARK(2);                                           // S1 wait
@@ -520,7 +540,7 @@ aggregate_kernel(const uint4* __restrict__ recs, uint32_t n, Table t, uint64_t e
                     tc.done = 0;
                     tc.nrep = 0;                                   // every warp has read the list length; reset it before the
                                                                    // next tile can arrive (its E phase starts right after S2)
-                    const uint32_t nt = tile_idx + tile_stride;
+                    const uint32_t nt = tc.next[it & 1u];
                     if (!kSketch && nt < n_tiles) { fence_proxy_async(); issue_tile_load(s, tc, recs, n, nt); }
                 }
             }
@@ -584,10 +604,10 @@ aggregate_kernel(const uint4* __restrict__ recs, uint32_t n, Table t, uint64_t e
         }
         team_sync(team);                                           // S2: nobody reads the tile buffer any more
         FA_PROF_MARK(6);                                           // S2 wait
+        tile_idx = tc.next[it & 1u];
         if (tid == 0) {
             if (kSketch) {                                         // the sketch update reads the keys in the reduce step: re-arm here
-                const uint32_t nt = tile_idx + tile_stride;
-                if (nt < n_tiles) { fence_proxy_async(); issue_tile_load(s, tc, recs, n, nt); }
+                if (tile_idx < n_tiles) { fence_proxy_async(); issue_tile_load(s, tc, recs, n, tile_idx); }
             }
         }
         FA_PROF_MARK(7);                                           // reductions
@@ -642,6 +662,22 @@ aggregate_kernel(const uint4* __restrict__ recs, uint32_t n, Table t, uint64_t e
         if (cs.n_insert) atomicAdd(&ctr->live, (unsigned long long)cs.n_insert);
         if (cs.n_spill) atomicAdd(&ctr->spills, (unsigned long long)cs.n_spill);
         if (cs.any_dirty) *reinterpret_cast<volatile unsigned long long*>(&ctr->dirty) = 1ull;
+        // every team of this CTA has made its last claim and its inserts are counted: the last CTA out zeroes the
+        // claim counter for the next launch and hands the live-flow count to the host
+        __threadfence();
+        unsigned int* const ticket = k1_exit_ticket(ctr);
+        if (atomicAdd(ticket, 1u) == gridDim.x - 1u) {
+            __threadfence();
+            *tile_claims = 0u;
+            *ticket = 0u;
+            if (ctr->live_ring) {
+                const unsigned long long seq = ctr->live_seq;
+                ctr->live_seq = seq + 1ull;
+                const unsigned long long live = *reinterpret_cast<volatile unsigned long long*>(&ctr->live);
+                *reinterpret_cast<volatile unsigned long long*>(&ctr->live_ring[seq % kLiveRing]) = live;
+                __threadfence_system();
+            }
+        }
     }
 }
 
@@ -662,6 +698,7 @@ __device__ __forceinline__ uint32_t scratch_home(uint64_t slot, uint32_t smask) 
 
 __global__ void fixup_scan_kernel(const uint4* __restrict__ recs, uint32_t n, Table t, Counters* ctr, FixupScratch* scratch,
                                   uint32_t smask, uint32_t opt) {
+    pdl_wait();
     if (*reinterpret_cast<volatile unsigned long long*>(&ctr->dirty) == 0ull) return;
     if (opt & 16u) n = min(n, (uint32_t)ctr->launch_n);
     for (uint32_t i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += gridDim.x * blockDim.x) {
@@ -698,6 +735,7 @@ __global__ void fixup_scan_kernel(const uint4* __restrict__ recs, uint32_t n, Ta
 
 __global__ void fixup_apply_kernel(const uint4* __restrict__ recs, Table t, uint64_t epoch, Counters* ctr,
                                    FixupScratch* scratch, uint32_t scratch_slots, unsigned int* ticket) {
+    pdl_wait();
     if (*reinterpret_cast<volatile unsigned long long*>(&ctr->dirty) == 0ull) return;
     uint32_t fixed = 0;
     for (uint32_t a = blockIdx.x * blockDim.x + threadIdx.x; a < scratch_slots; a += gridDim.x * blockDim.x) {
@@ -766,22 +804,24 @@ int launch_aggregate(const AggLaunch& a, cudaStream_t st) {
     const uint32_t n_tiles = (a.n + kTile - 1) / kTile;
     const int grid = (int)min((uint32_t)a.sm_count, (n_tiles + kTeams - 1) / kTeams);
     const bool dev_n = (a.opt & 16u) != 0;                 // a.n is an upper bound, the count is in ctr->launch_n
-#define FA_K1_ARGS a.recs, a.n, a.table, a.epoch, a.ctr, a.spill_idx, a.sk
-    if (a.prof)
-        aggregate_kernel<false, true, false><<<grid, kCtaThreads, smem, st>>>(FA_K1_ARGS, a.prof, a.opt);
-    else if (a.sk.cms && dev_n)
-        aggregate_kernel<true, false, true><<<grid, kCtaThreads, smem, st>>>(FA_K1_ARGS, nullptr, a.opt);
-    else if (a.sk.cms)
-        aggregate_kernel<true, false, false><<<grid, kCtaThreads, smem, st>>>(FA_K1_ARGS, nullptr, a.opt);
-    else if (dev_n)
-        aggregate_kernel<false, false, true><<<grid, kCtaThreads, smem, st>>>(FA_K1_ARGS, nullptr, a.opt);
-    else
-        aggregate_kernel<false, false, false><<<grid, kCtaThreads, smem, st>>>(FA_K1_ARGS, nullptr, a.opt);
-#undef FA_K1_ARGS
-    const int fgrid = a.sm_count * 2;
-    fixup_scan_kernel<<<fgrid, 256, 0, st>>>(a.recs, a.n, a.table, a.ctr, a.scratch, a.scratch_slots - 1, a.opt);
-    fixup_apply_kernel<<<fgrid, 256, 0, st>>>(a.recs, a.table, a.epoch, a.ctr, a.scratch, a.scratch_slots,
-                                              reinterpret_cast<unsigned int*>(&a.ctr->scratch[1]));
+    // The three kernels are launched with programmatic stream serialization: each may be scheduled while the kernel
+    // before it drains, and waits (pdl_wait) before it reads anything that kernel writes.
+    cudaLaunchAttribute pdl[1];
+    pdl[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
+    pdl[0].val.programmaticStreamSerializationAllowed = 1;
+    cudaLaunchConfig_t cfg{};
+    cfg.gridDim = dim3((unsigned)grid); cfg.blockDim = dim3(kCtaThreads); cfg.dynamicSmemBytes = (size_t)smem; cfg.stream = st;
+    cfg.attrs = pdl; cfg.numAttrs = 1;
+    auto k1 = aggregate_kernel<false, false, false>;
+    if (a.prof) k1 = aggregate_kernel<false, true, false>;
+    else if (a.sk.cms && dev_n) k1 = aggregate_kernel<true, false, true>;
+    else if (a.sk.cms) k1 = aggregate_kernel<true, false, false>;
+    else if (dev_n) k1 = aggregate_kernel<false, false, true>;
+    cudaLaunchKernelEx(&cfg, k1, a.recs, a.n, a.table, a.epoch, a.ctr, a.spill_idx, a.sk, a.prof, a.opt);
+    cfg.gridDim = dim3((unsigned)(a.sm_count * 2)); cfg.blockDim = dim3(256); cfg.dynamicSmemBytes = 0;
+    cudaLaunchKernelEx(&cfg, fixup_scan_kernel, a.recs, a.n, a.table, a.ctr, a.scratch, a.scratch_slots - 1, a.opt);
+    cudaLaunchKernelEx(&cfg, fixup_apply_kernel, a.recs, a.table, a.epoch, a.ctr, a.scratch, a.scratch_slots,
+                       reinterpret_cast<unsigned int*>(&a.ctr->scratch[1]));
     return 3;
 }
 #endif  // FA_HOST_EMUL

@@ -73,7 +73,13 @@ struct Counters {
     unsigned long long evict_out;     // output cursor of the evict kernel
     unsigned long long scratch[3];
     unsigned long long launch_n;      // record count of a launch whose size is only known on the device (opt bit 4)
+    // ACCOUNTER: the host's ring of live-flow counts (mapped pinned memory, kLiveRing entries; nullptr in KERNEL_MAP
+    // mode).  The last CTA of K1 number `live_seq` writes `live` into entry live_seq % kLiveRing, so the host reads
+    // each launch's count without a copy after it.
+    unsigned long long* live_ring;
+    unsigned long long live_seq;      // K1 launches that have written the ring
 };
+constexpr int kLiveRing = 8;
 
 // ------------------------------------------------------------------ hash spec (DESIGN.md §hash)
 FA_HD uint64_t fmix64(uint64_t x) {
@@ -213,6 +219,13 @@ __device__ __forceinline__ void red_max_u32(void* p, uint32_t v) { asm volatile(
 __device__ __forceinline__ void red_min_u32(void* p, uint32_t v) { asm volatile("red.global.min.u32 [%0], %1;" ::"l"(p), "r"(v) : "memory"); }
 
 __device__ __forceinline__ uint64_t u64_of(uint32_t lo, uint32_t hi) { return (uint64_t)lo | ((uint64_t)hi << 32); }
+
+// A kernel launched with programmatic stream serialization may start while the kernel before it on the stream is still
+// draining; it calls this before its first access to global memory that kernel may write, and waits there until that
+// kernel has completed and its writes are visible.  A no-op for a kernel launched without the attribute.
+__device__ __forceinline__ void pdl_wait() { asm volatile("griddepcontrol.wait;" ::: "memory"); }
+#else
+inline void pdl_wait() {}                     // host emulation of the tests: kernels run one after the other
 #endif  // __CUDACC__
 
 // ------------------------------------------------------------------ read-only table probe

@@ -182,8 +182,8 @@ struct fa_engine {
     // launch; unsynced_records bounds the flows that launches still in flight can add.
     uint64_t live_known = 0;
     uint64_t unsynced_records = 0;
-    static constexpr int kLiveRing = 8;
-    unsigned long long* h_live_ring = nullptr;   // pinned, kLiveRing entries
+    static constexpr int kLiveRing = fa::kLiveRing;
+    unsigned long long* h_live_ring = nullptr;   // mapped pinned, kLiveRing entries (ACCOUNTER: written by K1, Counters::live_ring)
     cudaEvent_t ev_live[kLiveRing] = {};
     uint32_t ring_n[kLiveRing] = {};
     uint32_t ring_head = 0, ring_tail = 0;       // monotonically increasing; slot = idx % kLiveRing
@@ -250,7 +250,11 @@ void retire_completed(fa_engine* e) {
     }
 }
 
-// Book-keeping after the launches of one chunk: asynchronous read-back of the live-flow count.
+// Book-keeping after the launches of one chunk: asynchronous read-back of the live-flow count.  In ACCOUNTER mode the
+// chunk was one K1 launch, whose last CTA writes the count into ring entry ring_tail % kLiveRing itself (every K1 launch
+// comes through here once, so the device's Counters::live_seq and ring_tail stay equal).  A KERNEL_MAP batch counts its
+// inserts in one or two resolve kernels of nine and has no ticket that ends after all of them, so the count is copied
+// after the batch.
 int note_launch(fa_engine* e, uint32_t n) {
     e->unsynced_records += n;
     e->st.records_ingested += n;
@@ -259,7 +263,8 @@ int note_launch(fa_engine* e, uint32_t n) {
         retire_completed(e);
     }
     const uint32_t s = e->ring_tail % fa_engine::kLiveRing;
-    CU(cudaMemcpyAsync(&e->h_live_ring[s], &e->d_ctr->live, 8, cudaMemcpyDeviceToHost, e->stream));
+    if (e->cfg.mode == FA_MODE_KERNEL_MAP)
+        CU(cudaMemcpyAsync(&e->h_live_ring[s], &e->d_ctr->live, 8, cudaMemcpyDeviceToHost, e->stream));
     CU(cudaEventRecord(e->ev_live[s], e->stream));
     e->ring_n[s] = n;
     e->ring_tail++;
@@ -600,7 +605,13 @@ int fa_create(const fa_config* cfg, fa_engine** out) {
     CU(cudaMemsetAsync(e->d_ctr, 0, sizeof(fa::Counters), e->stream));
     CU(cudaHostAlloc(&e->h_ctr, sizeof(fa::Counters), cudaHostAllocDefault));
     memset(e->h_ctr, 0, sizeof(fa::Counters));
-    CU(cudaHostAlloc(&e->h_live_ring, fa_engine::kLiveRing * 8, cudaHostAllocDefault));
+    CU(cudaHostAlloc(&e->h_live_ring, fa_engine::kLiveRing * 8, cudaHostAllocMapped));
+    if (cfg->mode != FA_MODE_KERNEL_MAP) {
+        // with unified addressing (every 64-bit process on sm_90) a mapped pinned buffer has the same address on the device
+        unsigned long long* ring = e->h_live_ring;
+        CU(cudaMemcpyAsync(&e->d_ctr->live_ring, &ring, sizeof ring, cudaMemcpyHostToDevice, e->stream));
+        CU(cudaStreamSynchronize(e->stream));
+    }
     for (int i = 0; i < fa_engine::kLiveRing; i++) CU(cudaEventCreateWithFlags(&e->ev_live[i], cudaEventDisableTiming));
 
     for (int i = 0; i < 2; i++) {
