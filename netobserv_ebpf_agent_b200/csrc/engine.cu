@@ -162,8 +162,8 @@ struct fa_engine {
     fa::ExpireCtr* h_expire_ctr = nullptr;    // pinned
     fa::GroupScratch group{};                 // fa_group_flows, under `mu`: group table (all zero between calls), list, counters
     fa::GroupCtr* h_group_ctr = nullptr;      // pinned
-    uint8_t* d_group_out = nullptr;           // ... and its staging of host-bound rows, group_out_cap rows
-    uint64_t group_out_cap = 0;
+    uint8_t* d_group_out = nullptr;           // ... and its staging of host-bound rows, group_out_bytes
+    uint64_t group_out_bytes = 0;
     uint32_t* d_hist_row_of = nullptr;        // fa_histogram_flows, under `mu`: row of each group, one u32 per group-table slot
     uint8_t* d_hist_out = nullptr;            // ... and its staging of host-bound rows, hist_out_bytes
     uint64_t hist_out_bytes = 0;
@@ -1107,14 +1107,10 @@ int fa_top_flows(fa_engine* e, uint32_t by, size_t k, const fa_evict_out* o, siz
     if (int rc = grow_staging(e, &e->top_stage, n, classify(o->records) != PTR_DEVICE, feats)) return rc;
     Blocks d;
     if (int rc = place_blocks(t, o, n, e->top_stage, st, &d)) return rc;
-    fa::TopMetric M{};
-    M.p = kmap ? t.met + (by == FA_TOP_BYTES ? fa::KM_BYTES : fa::KM_PACKETS) : reinterpret_cast<const uint8_t*>(t.hot) + (by == FA_TOP_BYTES ? 0 : 24);
-    M.stride = kmap ? fa::kMetLineBytes : fa::kHotBytes;
-    M.wide = by == FA_TOP_BYTES;
     CU(cudaMemsetAsync(s.state, 0, sizeof(fa::TopState), st));
     CU(cudaMemsetAsync(s.hist, 0, fa::kTopPasses * 256 * sizeof(unsigned), st));
     uint64_t launched = 0, d2h = 0;
-    launched += fa::launch_top_flows(t, kmap, M, n, live, s, d.rec, d.slot_of, e->sm_count, st);
+    launched += fa::launch_top_flows(t, kmap, by == FA_TOP_BYTES, n, live, s, d.rec, d.slot_of, e->sm_count, st);
     if (int rc = finish_blocks(e, t, o, n, d, /*clear=*/false, st, &launched, &d2h)) return rc;
     CU(cudaMemcpyAsync(e->h_top_state, s.state, sizeof(fa::TopState), cudaMemcpyDeviceToHost, st));
     CU(cudaStreamSynchronize(st));
@@ -1242,7 +1238,7 @@ int fa_expire_flows(fa_engine* e, uint64_t mono_now_ns, uint64_t idle_timeout_ns
         if (int rc = grow_staging(e, &e->expire_stage, n, classify(o->records) != PTR_DEVICE, feats)) return rc;
         Blocks d;
         if (int rc = place_blocks(t, o, n, e->expire_stage, st, &d)) return rc;
-        launched += fa::launch_expire_emit(t, kmap, s, n, d.rec, d.slot_of, e->sm_count, st);
+        launched += fa::launch_gather(t, kmap, s.list, 1u, n, false, d.rec, d.slot_of, e->sm_count, st);
         if (int rc = finish_blocks(e, t, o, n, d, /*clear=*/true, st, &launched, &d2h)) return rc;
         launched += fa::launch_expire_delete(t, s, n, live == e->slots, e->d_ctr, e->sm_count, st);
         CU(cudaGetLastError());
@@ -1257,17 +1253,19 @@ int fa_expire_flows(fa_engine* e, uint64_t mono_now_ns, uint64_t idle_timeout_ns
     return FA_OK;
 }
 
-// Exact roll-ups of the live flows by a key mask, read in place (evict.cu: launch_group_*), on the engine stream after
-// the queued folds: the scan folds every live flow into the group table and lists the groups, the host reads their
-// count (one wait), then one pass writes the listed groups' rows (device `out` in place, host `out` through the group
-// staging) and zeroes their slots, or only zeroes them when the rows are not wanted (FA_E_2BIG).  Either way the group
-// table is all zero again for the next call.  Nothing of the flow table or the counters is written.
-static int grow_group_out(fa_engine* e, uint64_t n) {
-    if (e->group_out_cap >= n) return FA_OK;
-    cudaFree(e->d_group_out); e->d_group_out = nullptr; e->group_out_cap = 0;
-    const uint64_t want = std::max<uint64_t>(n, std::min<uint64_t>(e->slots, 2 * n));
-    CU(cudaMalloc(&e->d_group_out, want * fa::kGroupRowBytes));
-    e->group_out_cap = want;
+// Device staging of host-bound rows (the group rows, the histogram rows): *buf grown to hold n rows of row_bytes, with
+// room for twice that up to one row per flow-table slot.  On failure no buffer and no pending CUDA error are left, so
+// the caller still clears the group table.
+static int grow_group_out(uint8_t** buf, uint64_t* have_bytes, uint64_t n, uint64_t row_bytes, uint64_t slots, const char* who) {
+    if (*have_bytes >= n * row_bytes) return FA_OK;
+    cudaFree(*buf); *buf = nullptr; *have_bytes = 0;
+    const uint64_t want = std::max<uint64_t>(n, std::min<uint64_t>(slots, 2 * n)) * row_bytes;
+    if (cudaMalloc(buf, want) != cudaSuccess) {
+        (void)cudaGetLastError();
+        *buf = nullptr;
+        return fail(FA_E_CUDA, "%s: no device memory for %llu B of staging", who, (unsigned long long)want);
+    }
+    *have_bytes = want;
     return FA_OK;
 }
 
@@ -1290,6 +1288,37 @@ static int grow_group_table(fa_engine* e, uint64_t live, bool with_row_of) {
     return FA_OK;
 }
 
+// The group scan fa_group_flows and fa_histogram_flows start with, on the engine stream after the queued folds: the
+// masked key (byte 39, padding, is ignored), the group table for `live` flows, the scan, and the group count (the one
+// wait).  A non-zero return ends the call at once.  Otherwise g->rc is FA_OK, FA_E_CUDA (more groups than live flows,
+// or folds without a slot) or FA_E_2BIG (more groups than cap), and in every case the caller clears the g->n listed
+// groups.
+struct GroupScan { fa::GroupMask m; uint64_t n, launched; int rc; };
+static int scan_groups(fa_engine* e, const char* who, const uint8_t key_mask[40], uint64_t live, size_t cap, bool with_row_of,
+                       GroupScan* g) {
+    memcpy(g->m.w, key_mask, fa::kKeyBytes);
+    g->m.w[4] &= 0x00FFFFFFFFFFFFFFull;
+    if (int rc = grow_group_table(e, live, with_row_of)) return rc;
+    const fa::GroupScratch s = e->group;
+    CU(cudaMemsetAsync(s.ctr, 0, sizeof(fa::GroupCtr), e->stream));
+    g->launched = fa::launch_group_scan(e->table, g->m, s, e->sm_count, e->stream);
+    CU(cudaGetLastError());
+    CU(cudaMemcpyAsync(e->h_group_ctr, s.ctr, sizeof(fa::GroupCtr), cudaMemcpyDeviceToHost, e->stream));
+    CU(cudaStreamSynchronize(e->stream));
+    g->n = e->h_group_ctr->n;
+    g->rc = FA_OK;
+    if (e->h_group_ctr->lost || g->n > live)
+        g->rc = fail(FA_E_CUDA, "%s: %llu groups of %llu live flows, %llu folds without a slot", who, (unsigned long long)g->n,
+                     (unsigned long long)live, e->h_group_ctr->lost);
+    else if (g->n > cap)
+        g->rc = fail(FA_E_2BIG, "%s: capacity %zu < %llu groups", who, cap, (unsigned long long)g->n);
+    return FA_OK;
+}
+
+// Exact roll-ups of the live flows by a key mask, read in place (evict.cu: launch_group_*): the group scan, then one
+// pass writes the listed groups' rows (device `out` in place, host `out` through the group staging) and zeroes their
+// slots, or only zeroes them when the rows are not wanted (FA_E_2BIG).  Either way the group table is all zero again for
+// the next call.  Nothing of the flow table or the counters is written.
 int fa_group_flows(fa_engine* e, const uint8_t key_mask[40], fa_flow_group* out, size_t cap, size_t* n_groups) {
     if (n_groups) *n_groups = 0;
     if (!e || !key_mask || !n_groups || (!out && cap)) return fail(FA_E_INVAL, "fa_group_flows: null argument");
@@ -1302,27 +1331,17 @@ int fa_group_flows(fa_engine* e, const uint8_t key_mask[40], fa_flow_group* out,
     const uint64_t live = e->live_known;
     if (live == 0) return FA_OK;
     cudaStream_t st = e->stream;
-    fa::GroupMask m;
-    memcpy(m.w, key_mask, fa::kKeyBytes);
-    m.w[4] &= 0x00FFFFFFFFFFFFFFull;                   // byte 39 (padding) is ignored
-    if (int rc = grow_group_table(e, live, false)) return rc;
+    GroupScan g;
+    if (int rc = scan_groups(e, "fa_group_flows", key_mask, live, cap, false, &g)) return rc;
     const fa::GroupScratch s = e->group;
-    CU(cudaMemsetAsync(s.ctr, 0, sizeof(fa::GroupCtr), st));
-    uint64_t launched = fa::launch_group_scan(e->table, m, s, e->sm_count, st);
-    CU(cudaGetLastError());
-    CU(cudaMemcpyAsync(e->h_group_ctr, s.ctr, sizeof(fa::GroupCtr), cudaMemcpyDeviceToHost, st));
-    CU(cudaStreamSynchronize(st));
-    const uint64_t n = e->h_group_ctr->n;
-    int rc = FA_OK;
-    if (e->h_group_ctr->lost || n > live)
-        rc = fail(FA_E_CUDA, "fa_group_flows: %llu groups of %llu live flows, %llu folds without a slot", (unsigned long long)n,
-                  (unsigned long long)live, e->h_group_ctr->lost);
-    else if (n > cap)
-        rc = fail(FA_E_2BIG, "fa_group_flows: capacity %zu < %llu groups", cap, (unsigned long long)n);
+    const uint64_t n = g.n;
+    uint64_t launched = g.launched;
+    int rc = g.rc;
     uint64_t* rows = nullptr;
     if (rc == FA_OK) {
         if (out_dev) rows = reinterpret_cast<uint64_t*>(out);
-        else if ((rc = grow_group_out(e, n)) == FA_OK) rows = reinterpret_cast<uint64_t*>(e->d_group_out);
+        else if ((rc = grow_group_out(&e->d_group_out, &e->group_out_bytes, n, fa::kGroupRowBytes, e->slots, "fa_group_flows")) == FA_OK)
+            rows = reinterpret_cast<uint64_t*>(e->d_group_out);
     }
     launched += fa::launch_group_emit(s, std::min<uint64_t>(n, s.mask + 1), rows, e->sm_count, st);   // rows == nullptr: clear only
     CU(cudaGetLastError());
@@ -1339,10 +1358,9 @@ int fa_group_flows(fa_engine* e, const uint8_t key_mask[40], fa_flow_group* out,
 }
 
 // Per-group histograms of one per-flow value (evict.cu: launch_hist_*), on the groups of fa_group_flows: the group scan
-// builds the groups and their flow counts, the host reads their count (the one wait), then the rows are zeroed (device
-// `out` in place, host `out` through the histogram staging), indexed by group, binned by a second scan of the live flows
-// and completed from the group table, which is zeroed after (FA_E_2BIG: only zeroed).  Nothing of the flow table or the
-// counters is written.
+// builds the groups and their flow counts, then the rows are zeroed (device `out` in place, host `out` through the
+// histogram staging), indexed by group, binned by a second scan of the live flows and completed from the group table,
+// which is zeroed after (FA_E_2BIG: only zeroed).  Nothing of the flow table or the counters is written.
 static_assert(FA_HIST_BYTES == fa::kHistBytes && FA_HIST_PACKETS == fa::kHistPackets && FA_HIST_DURATION == fa::kHistDuration &&
               FA_HIST_RTT == fa::kHistRtt && FA_HIST_DNS_LATENCY == fa::kHistDnsLatency, "FA_HIST_* values");
 static_assert(FA_HIST_MAX_BOUNDS == fa::kHistMaxBounds && sizeof(fa_hist_row) == fa::kHistHeadWords * 8 &&
@@ -1370,49 +1388,27 @@ int fa_histogram_flows(fa_engine* e, const uint8_t key_mask[40], uint32_t value,
     const uint64_t live = e->live_known;
     if (live == 0) return FA_OK;
     cudaStream_t st = e->stream;
-    fa::GroupMask m;
-    memcpy(m.w, key_mask, fa::kKeyBytes);
-    m.w[4] &= 0x00FFFFFFFFFFFFFFull;                   // byte 39 (padding) is ignored
     fa::HistParams h{};
     memcpy(h.bounds, bounds, n_bounds * sizeof(uint64_t));
     h.n_bounds = n_bounds;
     h.value = value;
     const uint64_t row_bytes = FA_HIST_ROW_BYTES(n_bounds);
-    if (int rc = grow_group_table(e, live, true)) return rc;
+    GroupScan g;
+    if (int rc = scan_groups(e, "fa_histogram_flows", key_mask, live, cap, true, &g)) return rc;
     const fa::GroupScratch s = e->group;
-    CU(cudaMemsetAsync(s.ctr, 0, sizeof(fa::GroupCtr), st));
-    uint64_t launched = fa::launch_group_scan(e->table, m, s, e->sm_count, st);
-    CU(cudaGetLastError());
-    CU(cudaMemcpyAsync(e->h_group_ctr, s.ctr, sizeof(fa::GroupCtr), cudaMemcpyDeviceToHost, st));
-    CU(cudaStreamSynchronize(st));
-    const uint64_t n = e->h_group_ctr->n;
-    int rc = FA_OK;
-    if (e->h_group_ctr->lost || n > live)
-        rc = fail(FA_E_CUDA, "fa_histogram_flows: %llu groups of %llu live flows, %llu folds without a slot", (unsigned long long)n,
-                  (unsigned long long)live, e->h_group_ctr->lost);
-    else if (n > cap)
-        rc = fail(FA_E_2BIG, "fa_histogram_flows: capacity %zu < %llu groups", cap, (unsigned long long)n);
+    const uint64_t n = g.n;
+    uint64_t launched = g.launched;
+    int rc = g.rc;
     uint64_t* rows = nullptr;
     if (rc == FA_OK) {
-        if (out_dev) {
-            rows = reinterpret_cast<uint64_t*>(out);
-        } else if (e->hist_out_bytes < n * row_bytes) {
-            cudaFree(e->d_hist_out); e->d_hist_out = nullptr; e->hist_out_bytes = 0;
-            const uint64_t want = std::max<uint64_t>(n, std::min<uint64_t>(e->slots, 2 * n)) * row_bytes;
-            if (cudaMalloc(&e->d_hist_out, want) == cudaSuccess) {
-                e->hist_out_bytes = want;
-            } else {                                   // the group table is still cleared below
-                (void)cudaGetLastError();
-                e->d_hist_out = nullptr;
-                rc = fail(FA_E_CUDA, "fa_histogram_flows: no device memory for %llu B of staging", (unsigned long long)want);
-            }
-        }
-        if (rc == FA_OK && !rows) rows = reinterpret_cast<uint64_t*>(e->d_hist_out);
+        if (out_dev) rows = reinterpret_cast<uint64_t*>(out);
+        else if ((rc = grow_group_out(&e->d_hist_out, &e->hist_out_bytes, n, row_bytes, e->slots, "fa_histogram_flows")) == FA_OK)
+            rows = reinterpret_cast<uint64_t*>(e->d_hist_out);
     }
     if (rows) {
         CU(cudaMemsetAsync(rows, 0, n * row_bytes, st));
         launched += fa::launch_hist_index(s, n, e->d_hist_row_of, e->sm_count, st);
-        launched += fa::launch_hist_scan(e->table, m, s, e->d_hist_row_of, h, rows, e->sm_count, st);
+        launched += fa::launch_hist_scan(e->table, g.m, s, e->d_hist_row_of, h, rows, e->sm_count, st);
         launched += fa::launch_hist_emit(s, n, n_bounds, rows, e->sm_count, st);
         CU(cudaGetLastError());
         CU(cudaMemcpyAsync(e->h_group_ctr, s.ctr, sizeof(fa::GroupCtr), cudaMemcpyDeviceToHost, st));

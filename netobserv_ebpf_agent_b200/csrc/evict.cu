@@ -111,6 +111,51 @@ evict_kernel(Table t, uint4* __restrict__ out, uint32_t* __restrict__ slot_of_ou
     }
 }
 
+// ---- what the live-table queries share --------------------------------------------------------------------------------
+// The row fa_evict_ex would return for `slot` now: its bytes, packets (widened), flags, start and end from the hot line
+// (ACCOUNTER) or the KERNEL_MAP metric line.  All five lie in the first 32-byte sector of that line, and the loads are
+// plain ones: a caller that uses one word reads one.  patched: start / end patched by the slot's feature lines as the
+// eviction patches them (feature_patch, kernels.cuh), before the other words are read.  Besides this reader, only the
+// record assembly (emit_record, km_emit_record) and the slot moves of fa_expire_flows (slot_clear, slot_move) know
+// these lines.
+struct RowVals { uint64_t bytes, packets, start, end; uint32_t flags; };
+__device__ __forceinline__ RowVals row_read(const Table& t, uint64_t slot, bool patched) {
+    const uint8_t* M = t.met + slot * kMetLineBytes;
+    const uint64_t* H = reinterpret_cast<const uint64_t*>(t.hot + slot * 2);   // bytes, nstart, end, packets | flags
+    RowVals r;
+    if (t.met) { r.start = km_ld64(M + KM_START); r.end = km_ld64(M + KM_END); }
+    else { r.start = 0ull - H[1]; r.end = H[2]; }                              // nstart = 0 - start; 0 stays 0
+    uint32_t eth = 0;                                                          // not part of RowVals: never read
+    if (patched) feature_patch(t, slot, r.start, r.end, eth);
+    if (t.met) { r.bytes = km_ld64(M + KM_BYTES); r.packets = km_ld32(M + KM_PACKETS); r.flags = km_ld16(M + KM_FLAGS); }
+    else { r.bytes = H[0]; r.packets = (uint32_t)H[3]; r.flags = (uint32_t)(H[3] >> 32) & 0xFFFFu; }
+    return r;
+}
+
+// Exclusive prefix of cnt over the warp and one cursor atomic for the warp's total: this lane's first index.  Every lane
+// of the warp calls it.
+__device__ __forceinline__ unsigned long long warp_reserve(uint32_t cnt, unsigned long long* cursor) {
+    const int lane = threadIdx.x & 31;
+    uint32_t incl = cnt;
+#pragma unroll
+    for (int d = 1; d < 32; d <<= 1) { const uint32_t v = __shfl_up_sync(0xFFFFFFFFu, incl, d); if (lane >= d) incl += v; }
+    const uint32_t total = __shfl_sync(0xFFFFFFFFu, incl, 31);
+    unsigned long long base = 0;
+    if (lane == 0 && total) base = atomicAdd(cursor, (unsigned long long)total);
+    base = __shfl_sync(0xFFFFFFFFu, base, 0);
+    return base + incl - cnt;
+}
+
+// Every thread owns one occupancy bitmap word per grid-stride step (a warp: 1024 slots in one coalesced load) and walks
+// its set bits.  n_words and the stride are multiples of 32, so the lanes of a warp take the same number of steps.
+#define FOR_OCC_WORDS(t, w) \
+    for (uint64_t w = blockIdx.x * (uint64_t)blockDim.x + threadIdx.x; w < (((t).mask + 1) >> 5); w += (uint64_t)gridDim.x * blockDim.x)
+
+// Blocks of 256 threads for a grid-stride loop over `threads` threads: no more than needed, at most 8 per SM.
+static int grid_for(uint64_t threads, int sm_count) {
+    const uint64_t blocks = (threads + 255) / 256, cap = (uint64_t)sm_count * 8;
+    return (int)(blocks < cap ? blocks : cap);
+}
 
 // ---- fa_top_flows: the exact top-k of the live flows, without removing or changing anything ------------------------
 // Rank order: metric descending, then slot hash ascending, then key bytes ascending.  A radix select over the 128-bit
@@ -126,9 +171,9 @@ FA_HD uint64_t bswap64(uint64_t x) {
     x = ((x & 0x0000FFFF0000FFFFull) << 16) | ((x >> 16) & 0x0000FFFF0000FFFFull);
     return (x << 32) | (x >> 32);
 }
-FA_HD uint64_t top_metric(const TopMetric& M, uint64_t slot) {
-    const uint8_t* p = M.p + slot * M.stride;
-    return M.wide ? *reinterpret_cast<const uint64_t*>(p) : (uint64_t)*reinterpret_cast<const uint32_t*>(p);
+__device__ __forceinline__ uint64_t top_metric(const Table& t, uint64_t slot, bool by_bytes) {
+    if (by_bytes) return row_read(t, slot, false).bytes;   // a branch, not a select: one load per flow
+    return row_read(t, slot, false).packets;
 }
 FA_HD uint64_t top_hash(const Table& t, uint64_t slot) {
     const uint64_t* L = reinterpret_cast<const uint64_t*>(t.ident) + slot * (kIdentBytes / 8);
@@ -162,16 +207,11 @@ FA_HD bool top_before(const Table& t, const TopEnt& a, const TopEnt& b) {
     return false;
 }
 
-// Every thread owns one bitmap word per grid-stride step (a warp: 1024 slots in one coalesced load) and walks its set
-// bits.  n_words and the stride are multiples of 32, so the lanes of a warp take the same number of steps.
-#define TOP_FOR_WORDS(t, w) \
-    for (uint64_t w = blockIdx.x * (uint64_t)blockDim.x + threadIdx.x; w < (((t).mask + 1) >> 5); w += (uint64_t)gridDim.x * blockDim.x)
-
-__global__ void __launch_bounds__(256) top_max_kernel(Table t, TopMetric M, TopState* st) {
+__global__ void __launch_bounds__(256) top_max_kernel(Table t, bool by_bytes, TopState* st) {
     unsigned long long mx = 0;
-    TOP_FOR_WORDS(t, w) {
+    FOR_OCC_WORDS(t, w) {
         for (uint32_t r = t.occ[w]; r; r &= r - 1) {
-            const uint64_t m = top_metric(M, w * 32 + (__ffs(r) - 1));
+            const uint64_t m = top_metric(t, w * 32 + (__ffs(r) - 1), by_bytes);
             mx = m > mx ? m : mx;
         }
     }
@@ -215,7 +255,7 @@ __global__ void top_resolve_kernel(TopState* st, const unsigned* hist, unsigned 
 }
 
 // Histogram of the next digit over the flows that match the prefix (256 bins in shared memory).
-__global__ void __launch_bounds__(256) top_hist_kernel(Table t, TopMetric M, const TopState* st, unsigned* hist) {
+__global__ void __launch_bounds__(256) top_hist_kernel(Table t, bool by_bytes, const TopState* st, unsigned* hist) {
     FA_DYN_SMEM(smem);
     unsigned* H = reinterpret_cast<unsigned*>(smem);
     const TopState S = *st;
@@ -223,10 +263,10 @@ __global__ void __launch_bounds__(256) top_hist_kernel(Table t, TopMetric M, con
     for (int b = threadIdx.x; b < 256; b += blockDim.x) H[b] = 0u;
     __syncthreads();
     const uint32_t p = S.pos - 8u;
-    TOP_FOR_WORDS(t, w) {
+    FOR_OCC_WORDS(t, w) {
         for (uint32_t r = t.occ[w]; r; r &= r - 1) {
             const uint64_t slot = w * 32 + (__ffs(r) - 1);
-            const uint64_t m = top_metric(M, slot);
+            const uint64_t m = top_metric(t, slot, by_bytes);
             uint64_t lo = 0;
             bool have_lo = false;
             if (top_cmp(t, slot, m, S, lo, have_lo) != 0) continue;
@@ -246,10 +286,9 @@ __global__ void __launch_bounds__(256) top_hist_kernel(Table t, TopMetric M, con
 }
 
 // Every flow at or above the prefix into ents (one cursor atomic per warp step); their count is above + n_cand.
-__global__ void __launch_bounds__(256) top_compact_kernel(Table t, TopMetric M, TopState* st, TopEnt* ents, unsigned long long cap) {
+__global__ void __launch_bounds__(256) top_compact_kernel(Table t, bool by_bytes, TopState* st, TopEnt* ents, unsigned long long cap) {
     const TopState S = *st;
-    const int lane = threadIdx.x & 31;
-    TOP_FOR_WORDS(t, w) {
+    FOR_OCC_WORDS(t, w) {
         const uint32_t bits = t.occ[w];
         uint32_t take = 0;
         for (uint32_t r = bits; r; r &= r - 1) {
@@ -257,23 +296,14 @@ __global__ void __launch_bounds__(256) top_compact_kernel(Table t, TopMetric M, 
             const uint64_t slot = w * 32 + b;
             uint64_t lo = 0;
             bool have_lo = false;
-            if (top_cmp(t, slot, top_metric(M, slot), S, lo, have_lo) >= 0) take |= 1u << b;
+            if (top_cmp(t, slot, top_metric(t, slot, by_bytes), S, lo, have_lo) >= 0) take |= 1u << b;
         }
-        const uint32_t cnt = __popc(take);
-        uint32_t incl = cnt;
-#pragma unroll
-        for (int d = 1; d < 32; d <<= 1) { const uint32_t v = __shfl_up_sync(0xFFFFFFFFu, incl, d); if (lane >= d) incl += v; }
-        const uint32_t total = __shfl_sync(0xFFFFFFFFu, incl, 31);
-        if (total == 0u) continue;
-        unsigned long long base = 0;
-        if (lane == 0) base = atomicAdd(&st->count, (unsigned long long)total);
-        base = __shfl_sync(0xFFFFFFFFu, base, 0);
-        unsigned long long at = base + incl - cnt;
+        unsigned long long at = warp_reserve(__popc(take), &st->count);
         for (uint32_t r = take; r; r &= r - 1, at++) {
             const uint64_t slot = w * 32 + (__ffs(r) - 1);
             if (at < cap) {
                 TopEnt E;
-                E.m = top_metric(M, slot); E.h = top_hash(t, slot); E.slot = (uint32_t)slot; E.pad = 0u;
+                E.m = top_metric(t, slot, by_bytes); E.h = top_hash(t, slot); E.slot = (uint32_t)slot; E.pad = 0u;
                 ents[at] = E;
             }
         }
@@ -321,8 +351,8 @@ __global__ void __launch_bounds__(256) top_merge_kernel(Table t, TopEnt* e, unsi
     }
 }
 
-// Row i of `out` from the flow at slots[i * stride]: the sorted fa_top_flows candidates (stride: one TopEnt) or the
-// fa_lookup_flows probe results (stride 1).  kNoSlot: no flow; the row is written all zero when zero_miss (a lookup
+// Row i of `out` from the flow at slots[i * stride]: the sorted fa_top_flows candidates (stride: one TopEnt), the
+// fa_lookup_flows probe results or the fa_expire_flows list (stride 1).  kNoSlot: no flow; the row is written all zero when zero_miss (a lookup
 // miss), else left unwritten (padding in the first n of top-k: fewer candidates than n, the host reports it).
 // slot_of_out (optional, for the feature pass): the row's slot, 0 without a flow (read only by the peek).
 // ACCOUNTER layout (emit_record, 4 flows per warp step) ...
@@ -356,6 +386,16 @@ __global__ void __launch_bounds__(256) gather_kmap_kernel(Table t, const uint32_
     }
 }
 
+// One text for the device and the host emulation (FA_LAUNCH): both kernels loop grid-stride.
+int launch_gather(const Table& t, bool kmap, const uint32_t* slots, uint32_t stride, uint64_t n, bool zero_miss,
+                  uint8_t* out_recs, uint32_t* slot_of_out, int sm_count, cudaStream_t st) {
+    if (!n) return 0;
+    if (kmap) FA_LAUNCH(gather_kmap_kernel, grid_for(n, sm_count), 256, 0, st, t, slots, stride, n, zero_miss, out_recs, slot_of_out);
+    else FA_LAUNCH(gather_kernel, grid_for(n * 8, sm_count), 256, 0, st, t, slots, stride, n, zero_miss,
+                   reinterpret_cast<uint4*>(out_recs), slot_of_out);
+    return 1;
+}
+
 #ifndef FA_HOST_EMUL
 int launch_evict(const Table& table, uint4* out_recs, uint32_t* slot_of_out,
                  unsigned long long cap, Counters* ctr, int sm_count, cudaStream_t st, bool drain) {
@@ -366,18 +406,18 @@ int launch_evict(const Table& table, uint4* out_recs, uint32_t* slot_of_out,
 #endif  // FA_HOST_EMUL
 
 // One text for the device and the host emulation (FA_LAUNCH): every kernel of the sequence loops grid-stride.
-int launch_top_flows(const Table& t, bool kmap, const TopMetric& M, uint64_t n, uint64_t live, const TopScratch& s,
+int launch_top_flows(const Table& t, bool kmap, bool by_bytes, uint64_t n, uint64_t live, const TopScratch& s,
                      uint8_t* out_recs, uint32_t* slot_of_out, int sm_count, cudaStream_t st) {
     const int grid = sm_count * 8;
     const size_t tile_smem = kTopSortTile * sizeof(TopEnt);
     int launches = 0;
-    FA_LAUNCH(top_max_kernel, grid, 256, 0, st, t, M, s.state);
+    FA_LAUNCH(top_max_kernel, grid, 256, 0, st, t, by_bytes, s.state);
     FA_LAUNCH(top_resolve_kernel, 1, 32, 0, st, s.state, nullptr, n, live, s.cap);
     for (int p = 0; p < kTopPasses; p++) {                 // fixed sequence: passes after the last needed one exit at once
-        FA_LAUNCH(top_hist_kernel, grid, 256, 256 * sizeof(unsigned), st, t, M, s.state, s.hist + p * 256);
+        FA_LAUNCH(top_hist_kernel, grid, 256, 256 * sizeof(unsigned), st, t, by_bytes, s.state, s.hist + p * 256);
         FA_LAUNCH(top_resolve_kernel, 1, 32, 0, st, s.state, s.hist + p * 256, n, live, s.cap);
     }
-    FA_LAUNCH(top_compact_kernel, grid, 256, 0, st, t, M, s.state, s.ents, s.cap);
+    FA_LAUNCH(top_compact_kernel, grid, 256, 0, st, t, by_bytes, s.state, s.ents, s.cap);
     launches += 3 + 2 * kTopPasses;
     const unsigned tiles = (unsigned)(s.cap / kTopSortTile);
     FA_LAUNCH(top_sort_tile_kernel, tiles, kTopSortTile / 2, tile_smem, st, t, s.ents, s.state, s.cap, 0ull);
@@ -390,9 +430,7 @@ int launch_top_flows(const Table& t, bool kmap, const TopMetric& M, uint64_t n, 
     }
     const uint32_t* ent_slots = reinterpret_cast<const uint32_t*>(reinterpret_cast<const uint8_t*>(s.ents) + offsetof(TopEnt, slot));
     const uint32_t ent_stride = sizeof(TopEnt) / sizeof(uint32_t);
-    if (kmap) FA_LAUNCH(gather_kmap_kernel, grid, 256, 0, st, t, ent_slots, ent_stride, n, false, out_recs, slot_of_out);
-    else FA_LAUNCH(gather_kernel, grid, 256, 0, st, t, ent_slots, ent_stride, n, false, reinterpret_cast<uint4*>(out_recs), slot_of_out);
-    return launches + 1;
+    return launches + launch_gather(t, kmap, ent_slots, ent_stride, n, false, out_recs, slot_of_out, sm_count, st);
 }
 
 // ---- fa_lookup_flows: exact point lookups of live flows by key, without removing or changing anything -------------
@@ -426,18 +464,13 @@ __global__ void __launch_bounds__(256) lookup_probe_kernel(Table t, const uint64
 int launch_lookup_flows(const Table& t, bool kmap, const uint64_t* keys, uint64_t n, uint32_t* slots, uint8_t* found,
                         unsigned long long* hits, uint8_t* out_recs, int sm_count, cudaStream_t st) {
     if (!n) return 0;
-    const uint64_t cap = (uint64_t)sm_count * 8;
-    const uint64_t per_key = (n + 255) / 256, per_lanes = (n * 8 + 255) / 256;      // a thread per key / 8 lanes per row
-    const int g_probe = (int)(per_key < cap ? per_key : cap), g_rows = (int)(per_lanes < cap ? per_lanes : cap);
-    FA_LAUNCH(lookup_probe_kernel, g_probe, 256, 0, st, t, keys, n, slots, found, hits);
-    if (kmap) FA_LAUNCH(gather_kmap_kernel, g_probe, 256, 0, st, t, slots, 1u, n, true, out_recs, nullptr);
-    else FA_LAUNCH(gather_kernel, g_rows, 256, 0, st, t, slots, 1u, n, true, reinterpret_cast<uint4*>(out_recs), nullptr);
-    return 2;
+    FA_LAUNCH(lookup_probe_kernel, grid_for(n, sm_count), 256, 0, st, t, keys, n, slots, found, hits);
+    return 1 + launch_gather(t, kmap, slots, 1u, n, true, out_recs, nullptr, sm_count, st);
 }
 
 // ---- fa_expire_flows: remove only the flows past an idle or active timeout, in place -------------------------------
 // Mark (bitmap-driven, like top_hist_kernel): each live flow's row start / end, patched by its feature lines as the
-// eviction patches them, against the two timeouts -> expire bitmap + slot list.  Emit: the gather of fa_lookup_flows
+// eviction patches them, against the two timeouts -> expire bitmap + slot list.  Emit: launch_gather
 // over the list, then the clearing feature pass.  Delete: a cluster is a maximal cyclic run of occupied slots; its
 // bounds were EMPTY before the call and stay EMPTY, so clusters are independent and one thread takes each cluster that
 // holds an expiring flow: it clears the expiring slots, then vacates each survivor in cluster order and re-inserts it
@@ -450,44 +483,14 @@ __device__ __forceinline__ bool bit_at(const uint32_t* bm, uint64_t s) { return 
 __device__ __forceinline__ bool expire_due(uint64_t now, uint64_t ts, uint64_t timeout) {
     return timeout != 0 && (int64_t)(now - ts) >= (int64_t)timeout;   // signed, as time.Duration: a zero ts is infinitely old
 }
-// The start / end of the row fa_evict_ex would return for `slot` now: the hot line (ACCOUNTER) or the metric line
-// (KERNEL_MAP), patched with the effects of its feature lines in the eviction's order (evict_features_kernel).
-__device__ __forceinline__ void row_times(const Table& t, uint64_t slot, uint64_t& bs, uint64_t& be) {
-    if (t.met) {
-        const uint8_t* M = t.met + slot * kMetLineBytes;
-        bs = km_ld64(M + KM_START); be = km_ld64(M + KM_END);
-    } else {
-        const uint64_t* H = reinterpret_cast<const uint64_t*>(t.hot + slot * 2);
-        bs = 0ull - H[1]; be = H[2];                               // nstart = 0 - start; 0 stays 0
-    }
-    uint32_t beth = 0;
-    if (t.feat_dns) { const uint64_t* S = reinterpret_cast<const uint64_t*>(t.feat_dns + slot * kDnsState); if (S[0]) build_base(bs, be, beth, S[4], S[5], 0); }
-    if (t.feat_drop) { const uint64_t* S = reinterpret_cast<const uint64_t*>(t.feat_drop + slot * kDropState); if (S[0]) build_base(bs, be, beth, S[6], S[7], 0); }
-    if (t.feat_add) { const uint64_t* S = reinterpret_cast<const uint64_t*>(t.feat_add + slot * kAddState); if (S[0]) build_base(bs, be, beth, S[3], S[4], 0); }
-}
-// Exclusive prefix of cnt over the warp and one cursor atomic for the warp's total: this lane's first index.  Every lane
-// of the warp calls it.
-__device__ __forceinline__ unsigned long long warp_reserve(uint32_t cnt, unsigned long long* cursor) {
-    const int lane = threadIdx.x & 31;
-    uint32_t incl = cnt;
-#pragma unroll
-    for (int d = 1; d < 32; d <<= 1) { const uint32_t v = __shfl_up_sync(0xFFFFFFFFu, incl, d); if (lane >= d) incl += v; }
-    const uint32_t total = __shfl_sync(0xFFFFFFFFu, incl, 31);
-    unsigned long long base = 0;
-    if (lane == 0 && total) base = atomicAdd(cursor, (unsigned long long)total);
-    base = __shfl_sync(0xFFFFFFFFu, base, 0);
-    return base + incl - cnt;
-}
-
 __global__ void __launch_bounds__(256) expire_mark_kernel(Table t, uint64_t now, uint64_t idle, uint64_t active, uint32_t* __restrict__ bm,
                                                           uint32_t* __restrict__ list, unsigned long long cap, ExpireCtr* c) {
-    TOP_FOR_WORDS(t, w) {
+    FOR_OCC_WORDS(t, w) {
         uint32_t bits = 0;
         for (uint32_t r = t.occ[w]; r; r &= r - 1) {
             const int b = __ffs(r) - 1;
-            uint64_t s, e;
-            row_times(t, w * 32 + b, s, e);
-            if (expire_due(now, e, idle) || expire_due(now, s, active)) bits |= 1u << b;
+            const RowVals v = row_read(t, w * 32 + b, true);
+            if (expire_due(now, v.end, idle) || expire_due(now, v.start, active)) bits |= 1u << b;
         }
         bm[w] = bits;                                              // the thread owns the word: every word is written
         unsigned long long at = warp_reserve(__popc(bits), &c->n);
@@ -501,7 +504,7 @@ __global__ void __launch_bounds__(256) expire_mark_kernel(Table t, uint64_t now,
 __global__ void __launch_bounds__(256) expire_clusters_kernel(Table t, const uint32_t* __restrict__ bm, uint32_t* __restrict__ starts,
                                                               ExpireCtr* c) {
     const uint64_t n_words = (t.mask + 1) >> 5;
-    TOP_FOR_WORDS(t, w) {
+    FOR_OCC_WORDS(t, w) {
         const uint32_t o = t.occ[w], prev = t.occ[(w + n_words - 1) & (n_words - 1)];   // wraps at the last slot
         uint32_t take = 0;
         for (uint32_t r = o & ~((o << 1) | (prev >> 31)); r; r &= r - 1) {
@@ -599,17 +602,6 @@ int launch_expire_mark(const Table& t, uint64_t now, uint64_t idle, uint64_t act
     return 1;
 }
 
-int launch_expire_emit(const Table& t, bool kmap, const ExpireScratch& s, uint64_t n, uint8_t* out_recs, uint32_t* slot_of_out,
-                       int sm_count, cudaStream_t st) {
-    if (!n) return 0;
-    const uint64_t cap = (uint64_t)sm_count * 8;
-    const uint64_t per_row = (n + 255) / 256, per_lanes = (n * 8 + 255) / 256;     // a thread per row / 8 lanes per row
-    if (kmap) FA_LAUNCH(gather_kmap_kernel, (int)(per_row < cap ? per_row : cap), 256, 0, st, t, s.list, 1u, n, false, out_recs, slot_of_out);
-    else FA_LAUNCH(gather_kernel, (int)(per_lanes < cap ? per_lanes : cap), 256, 0, st, t, s.list, 1u, n, false,
-                   reinterpret_cast<uint4*>(out_recs), slot_of_out);
-    return 1;
-}
-
 int launch_expire_delete(const Table& t, const ExpireScratch& s, uint64_t n, bool full, Counters* ctr, int sm_count,
                          cudaStream_t st) {
     if (!n) return 0;
@@ -624,11 +616,10 @@ int launch_expire_delete(const Table& t, const ExpireScratch& s, uint64_t n, boo
 }
 
 // ---- fa_group_flows: exact roll-ups of the live flows by a key mask, without removing or changing anything --------
-// Scan (bitmap-driven, like expire_mark_kernel): each live flow's masked key and its row values (bytes, packets and
-// flags from the hot or metric line, start / end from row_times, so with the eviction's feature patch).  The lanes of
-// a warp take one flow each per round; the lanes with an equal masked key (every one of its ten 32-bit words: distinct
-// keys can share a premix) form a peer set, and one leader per set folds the set's sum into the group table.  Emit /
-// clear: one thread per listed group writes its row and zeroes its slot.
+// Scan (bitmap-driven, like expire_mark_kernel): each live flow's masked key and its row values (row_read with the
+// eviction's feature patch).  The lanes of a warp take one flow each per round; the lanes with an equal masked
+// key (every one of its ten 32-bit words: distinct keys can share a premix) form a peer set, and one leader per set
+// folds the set's sum into the group table.  Emit / clear: one thread per listed group writes its row and zeroes its slot.
 //
 // Group-table slot (12 u64): [0, 5) the group key, [5] state (0 EMPTY, kGroupWriting, kGroupPublished), [6] flows,
 // [7] bytes, [8] packets, [9] nstart = 0 - start (max: the smallest non-zero start, 0 if none), [10] end (max),
@@ -637,22 +628,6 @@ int launch_expire_delete(const Table& t, const ExpireScratch& s, uint64_t n, boo
 constexpr unsigned long long kGroupWriting = 1ull, kGroupPublished = 2ull;
 
 struct GroupVals { uint64_t bytes, packets, nstart, end; uint32_t flags; };
-
-// The fields of the row fa_evict_ex would return for `slot` now that fa_flow_group sums (packets widened to 64 bits).
-__device__ __forceinline__ GroupVals group_row(const Table& t, uint64_t slot) {
-    GroupVals v;
-    uint64_t s, e;
-    row_times(t, slot, s, e);
-    v.nstart = 0ull - s; v.end = e;
-    if (t.met) {
-        const uint8_t* M = t.met + slot * kMetLineBytes;
-        v.bytes = km_ld64(M + KM_BYTES); v.packets = km_ld32(M + KM_PACKETS); v.flags = km_ld16(M + KM_FLAGS);
-    } else {
-        const uint64_t* H = reinterpret_cast<const uint64_t*>(t.hot + slot * 2);
-        v.bytes = H[0]; v.packets = (uint32_t)H[3]; v.flags = (uint32_t)(H[3] >> 32) & 0xFFFFu;
-    }
-    return v;
-}
 
 __device__ __forceinline__ void group_add(unsigned long long* G, uint64_t flows, const GroupVals& v) {
     red_add_u64(G + 6, flows);
@@ -700,7 +675,7 @@ __device__ __forceinline__ bool group_fold(const GroupScratch& s, const uint64_t
 
 __global__ void __launch_bounds__(256) group_scan_kernel(Table t, GroupMask m, GroupScratch s) {
     const int lane = threadIdx.x & 31;
-    TOP_FOR_WORDS(t, w) {
+    FOR_OCC_WORDS(t, w) {
         uint32_t r = t.occ[w];
         while (__any_sync(0xFFFFFFFFu, r != 0u)) {             // converged rounds: at most one flow per lane
             const bool have = r != 0u;
@@ -712,7 +687,8 @@ __global__ void __launch_bounds__(256) group_scan_kernel(Table t, GroupMask m, G
                 const uint64_t* L = reinterpret_cast<const uint64_t*>(t.ident) + slot * (kIdentBytes / 8);
 #pragma unroll
                 for (int i = 0; i < 5; i++) k[i] = L[i] & m.w[i];
-                v = group_row(t, slot);
+                const RowVals r = row_read(t, slot, true);
+                v = GroupVals{r.bytes, r.packets, 0ull - r.start, r.end, r.flags};
             }
             const uint32_t active = __ballot_sync(0xFFFFFFFFu, have);
             uint32_t peers = active;
@@ -774,8 +750,7 @@ int launch_group_scan(const Table& t, const GroupMask& m, const GroupScratch& s,
 
 int launch_group_emit(const GroupScratch& s, uint64_t n, uint64_t* out, int sm_count, cudaStream_t st) {
     if (!n) return 0;
-    const uint64_t cap = (uint64_t)sm_count * 8, per_row = (n + 255) / 256;
-    FA_LAUNCH(group_emit_kernel, (int)(per_row < cap ? per_row : cap), 256, 0, st, s, (unsigned long long)n, out);
+    FA_LAUNCH(group_emit_kernel, grid_for(n, sm_count), 256, 0, st, s, (unsigned long long)n, out);
     return 1;
 }
 
@@ -795,20 +770,14 @@ constexpr uint64_t kHistNoGroup = ~0ull;
 // rules: duration needs a start, RTT a non-zero flow_rtt, DNS latency a DNS block with a non-zero id).
 __device__ __forceinline__ bool hist_value(const Table& t, uint64_t slot, uint32_t which, uint64_t& v) {
     if (which == kHistBytes || which == kHistPackets) {
-        if (t.met) {
-            const uint8_t* M = t.met + slot * kMetLineBytes;
-            v = which == kHistBytes ? km_ld64(M + KM_BYTES) : km_ld32(M + KM_PACKETS);
-        } else {
-            const uint64_t* H = reinterpret_cast<const uint64_t*>(t.hot + slot * 2);
-            v = which == kHistBytes ? H[0] : (uint32_t)H[3];
-        }
+        const RowVals r = row_read(t, slot, false);
+        v = which == kHistBytes ? r.bytes : r.packets;
         return true;
     }
     if (which == kHistDuration) {
-        uint64_t s, e;
-        row_times(t, slot, s, e);
-        v = e >= s ? e - s : 0ull;
-        return s != 0;
+        const RowVals r = row_read(t, slot, true);
+        v = r.end >= r.start ? r.end - r.start : 0ull;
+        return r.start != 0;
     }
     if (which == kHistRtt) {
         const uint64_t* S = reinterpret_cast<const uint64_t*>(t.feat_add + slot * kAddState);
@@ -848,7 +817,7 @@ __global__ void __launch_bounds__(256) hist_scan_kernel(Table t, GroupMask m, Gr
     __syncthreads();
     const int lane = threadIdx.x & 31;
     const uint64_t row_words = kHistHeadWords + h.n_bounds + 1;
-    TOP_FOR_WORDS(t, w) {
+    FOR_OCC_WORDS(t, w) {
         uint32_t r = t.occ[w];
         while (__any_sync(0xFFFFFFFFu, r != 0u)) {             // converged rounds: at most one flow per lane
             bool have = false;
@@ -910,8 +879,7 @@ __global__ void __launch_bounds__(256) hist_emit_kernel(GroupScratch s, unsigned
 
 int launch_hist_index(const GroupScratch& s, uint64_t n, uint32_t* row_of, int sm_count, cudaStream_t st) {
     if (!n) return 0;
-    const uint64_t cap = (uint64_t)sm_count * 8, per_row = (n + 255) / 256;
-    FA_LAUNCH(hist_index_kernel, (int)(per_row < cap ? per_row : cap), 256, 0, st, s, (unsigned long long)n, row_of);
+    FA_LAUNCH(hist_index_kernel, grid_for(n, sm_count), 256, 0, st, s, (unsigned long long)n, row_of);
     return 1;
 }
 
@@ -924,8 +892,7 @@ int launch_hist_scan(const Table& t, const GroupMask& m, const GroupScratch& s, 
 
 int launch_hist_emit(const GroupScratch& s, uint64_t n, uint32_t n_bounds, uint64_t* rows, int sm_count, cudaStream_t st) {
     if (!n) return 0;
-    const uint64_t cap = (uint64_t)sm_count * 8, per_row = (n + 255) / 256;
-    FA_LAUNCH(hist_emit_kernel, (int)(per_row < cap ? per_row : cap), 256, 0, st, s, (unsigned long long)n, n_bounds,
+    FA_LAUNCH(hist_emit_kernel, grid_for(n, sm_count), 256, 0, st, s, (unsigned long long)n, n_bounds,
               reinterpret_cast<unsigned long long*>(rows));
     return 1;
 }

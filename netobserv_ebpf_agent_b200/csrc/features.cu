@@ -395,11 +395,12 @@ int launch_feature_fold(int kind, const uint8_t* recs, uint32_t n, const Table& 
 }
 #endif  // FA_HOST_EMUL
 
-// ---- eviction: patch the base with the feature effects (build_base, kernels.cuh), emit and clear the feature blocks --
+// ---- eviction: patch the base with the feature effects (feature_patch, kernels.cuh), emit and clear the feature blocks
 // kClear = false: the fa_top_flows / fa_lookup_flows peek, which emits the same rows and leaves the feature lines as
-// they are; a row whose slot is kNoSlot (a lookup miss) gets zero feature rows and present = 0.
+// they are; a row whose slot is kNoSlot (a lookup miss) gets zero feature rows and present = 0.  Launched as 8 CTAs of
+// 256 threads per SM: the bound keeps them all resident (32 registers).
 template <bool kClear = true>
-__global__ void evict_features_kernel(Table t, const uint32_t* __restrict__ slot_of_out, unsigned long long n_out,
+__global__ void __launch_bounds__(256, 8) evict_features_kernel(Table t, const uint32_t* __restrict__ slot_of_out, unsigned long long n_out,
                                       uint8_t* __restrict__ out_recs, uint8_t* __restrict__ out_dns,
                                       uint8_t* __restrict__ out_add, uint8_t* __restrict__ out_drop,
                                       unsigned long long* __restrict__ out_rtt_min, uint8_t* __restrict__ out_present) {
@@ -417,12 +418,10 @@ __global__ void evict_features_kernel(Table t, const uint32_t* __restrict__ slot
         uint8_t* O = out_recs + i * kRecBytes;
         uint64_t bs = *reinterpret_cast<uint64_t*>(O + R_START), be = *reinterpret_cast<uint64_t*>(O + R_END);
         uint32_t beth = *reinterpret_cast<uint16_t*>(O + R_ETH);
-        uint8_t present = 0;
-        if (t.feat_dns) {                                 // DNS first, then additional: tracer.go:1098-1106,1143-1151
+        const uint32_t present = feature_patch(t, slot, bs, be, beth);
+        if (t.feat_dns) {
             uint64_t* S = reinterpret_cast<uint64_t*>(reinterpret_cast<uint8_t*>(t.feat_dns) + (size_t)slot * (kDnsState * 16));
-            if (S[0] != 0) {
-                present |= 1;
-                build_base(bs, be, beth, S[4], S[5], S[6]);
+            if (present & 1) {
                 if (out_dns) {
                     uint8_t* D = out_dns + i * 64;
                     const uint8_t* Sb = reinterpret_cast<const uint8_t*>(S);
@@ -436,7 +435,7 @@ __global__ void evict_features_kernel(Table t, const uint32_t* __restrict__ slot
                     for (int b = 0; b < 32; b++) D[31 + b] = Sb[80 + b];
                     D[63] = 0;
                 }
-if (kClear) {
+                if (kClear) {
 #pragma unroll
                     for (int c = 0; c < 16; c++) S[c] = 0ull;
                 }
@@ -444,11 +443,9 @@ if (kClear) {
                 for (int c = 0; c < 8; c++) reinterpret_cast<uint64_t*>(out_dns + i * 64)[c] = 0ull;
             }
         }
-        if (t.feat_drop) {                                // packet drops come second (tracer.go:1107-1115)
+        if (t.feat_drop) {
             uint64_t* S = reinterpret_cast<uint64_t*>(reinterpret_cast<uint8_t*>(t.feat_drop) + (size_t)slot * (kDropState * 16));
-            if (S[0] != 0) {
-                present |= 4;
-                build_base(bs, be, beth, S[6], S[7], S[8]);
+            if (present & 4) {
                 if (out_drop) {
                     uint8_t* D = out_drop + i * 32;
                     const uint8_t* Sb = reinterpret_cast<const uint8_t*>(S);
@@ -461,7 +458,7 @@ if (kClear) {
                     *reinterpret_cast<uint16_t*>(D + 26) = *reinterpret_cast<const uint16_t*>(Sb + 44);              // first.eth
                     *reinterpret_cast<uint32_t*>(D + 28) = (uint32_t)(S[4] & 0xFFu);          // latest_state: last non-zero; padding
                 }
-if (kClear) {
+                if (kClear) {
 #pragma unroll
                     for (int c = 0; c < 12; c++) S[c] = 0ull;
                 }
@@ -472,10 +469,8 @@ if (kClear) {
         if (out_rtt_min) out_rtt_min[i] = 0ull;
         if (t.feat_add) {
             uint64_t* S = reinterpret_cast<uint64_t*>(reinterpret_cast<uint8_t*>(t.feat_add) + (size_t)slot * (kAddState * 16));
-            if (S[0] != 0) {
-                present |= 2;
+            if (present & 2) {
                 if (out_rtt_min) out_rtt_min[i] = S[9] ? ~S[9] : 0ull;                       // extension: smallest non-zero RTT
-                build_base(bs, be, beth, S[3], S[4], S[5]);
                 if (out_add) {
                     uint8_t* A = out_add + i * 32;
                     *reinterpret_cast<uint64_t*>(A + 0) = S[6];                              // first.start
@@ -487,7 +482,7 @@ if (kClear) {
                     A[30] = (uint8_t)(ip & 1u);
                     A[31] = 0;
                 }
-if (kClear) {
+                if (kClear) {
 #pragma unroll
                     for (int c = 0; c < 10; c++) S[c] = 0ull;
                 }

@@ -67,13 +67,31 @@ constexpr int kAddState = 5;
 constexpr int kDnsState = 8;
 constexpr int kDropState = 6;
 #if defined(__CUDACC__) || defined(FA_HOST_EMUL)
-// buildBaseFromAdditional (flow_content.go:63-74) with the fold of all samples of one feature: the eviction's base patch
-// (evict_features_kernel) and the timestamps fa_expire_flows tests
+// buildBaseFromAdditional (flow_content.go:63-74) with the fold of all samples of one feature
 __device__ __forceinline__ void build_base(uint64_t& bs, uint64_t& be, uint32_t& beth, uint64_t nfs, uint64_t fe, uint64_t neth) {
     const uint64_t s = 0ull - nfs;                       // min non-zero start of the samples, 0 if none
     if (bs == 0 || (bs > s && s != 0)) bs = s;
     if (be == 0 || be < fe) be = fe;
     if (beth == 0 && neth != 0) beth = (uint32_t)(~neth) & 0xFFFFu;
+}
+// The eviction's patch of a row's start / end / eth_protocol by the non-empty feature lines of `slot`, in its order: DNS,
+// then packet drops, then additional (tracer.go:1098-1115,1143-1151).  Returns the present bits: 1 DNS, 2 additional,
+// 4 drops.  The eviction's feature pass (evict_features_kernel) and the live-table queries' row reader (evict.cu).
+__device__ __forceinline__ uint32_t feature_patch(const Table& t, uint64_t slot, uint64_t& bs, uint64_t& be, uint32_t& beth) {
+    uint32_t present = 0;
+    if (t.feat_dns) {                                    // nfs, fe, neth: words 4, 5, 6
+        const uint64_t* S = reinterpret_cast<const uint64_t*>(t.feat_dns + slot * kDnsState);
+        if (S[0]) { present |= 1; build_base(bs, be, beth, S[4], S[5], S[6]); }
+    }
+    if (t.feat_drop) {                                   // words 6, 7, 8
+        const uint64_t* S = reinterpret_cast<const uint64_t*>(t.feat_drop + slot * kDropState);
+        if (S[0]) { present |= 4; build_base(bs, be, beth, S[6], S[7], S[8]); }
+    }
+    if (t.feat_add) {                                    // words 3, 4, 5
+        const uint64_t* S = reinterpret_cast<const uint64_t*>(t.feat_add + slot * kAddState);
+        if (S[0]) { present |= 2; build_base(bs, be, beth, S[3], S[4], S[5]); }
+    }
+    return present;
 }
 #endif
 int launch_evict_features(const Table& t, const uint32_t* slot_of_out, unsigned long long n_out, uint8_t* out_recs,
@@ -84,9 +102,13 @@ int launch_peek_features(const Table& t, const uint32_t* slot_of_out, unsigned l
                          uint8_t* out_dns, uint8_t* out_add, uint8_t* out_drop, unsigned long long* out_rtt_min,
                          uint8_t* out_present, int sm_count, cudaStream_t st);
 
+// Rows of the n flows at slots[i * stride] into out_recs (device, n x 144 B), their slots into slot_of_out (optional, for
+// the feature pass; 0 without a flow).  A slot kNoSlot is no flow: its row is written all zero when zero_miss, else left
+// as it is.  kmap: KERNEL_MAP record layout.
+int launch_gather(const Table& t, bool kmap, const uint32_t* slots, uint32_t stride, uint64_t n, bool zero_miss,
+                  uint8_t* out_recs, uint32_t* slot_of_out, int sm_count, cudaStream_t st);
+
 // fa_top_flows (evict.cu): radix select over the composite (metric, ~slot hash), compaction, sort, gather.
-// Where a flow's metric is: the u64 (wide) or u32 at p + slot * stride (the hot line or the KERNEL_MAP metric line).
-struct TopMetric { const uint8_t* p; uint32_t stride; uint32_t wide; };
 // one compacted candidate; slot == kTopNoSlot marks the padding that sorts last
 struct TopEnt { unsigned long long m, h; uint32_t slot, pad; };
 constexpr uint32_t kTopNoSlot = kNoSlot;
@@ -113,8 +135,9 @@ struct TopScratch {
     uint64_t cap;
 };
 // The n (<= live) highest-ranked live flows of `t` into out_recs (device, n x 144 B) in rank order, and their slots into
-// slot_of_out (optional, for the feature pass).  kmap: KERNEL_MAP record layout.  Nothing in `t` changes.
-int launch_top_flows(const Table& t, bool kmap, const TopMetric& M, uint64_t n, uint64_t live, const TopScratch& s,
+// slot_of_out (optional, for the feature pass).  by_bytes: rank by bytes, else by packets.  kmap: KERNEL_MAP record
+// layout.  Nothing in `t` changes.
+int launch_top_flows(const Table& t, bool kmap, bool by_bytes, uint64_t n, uint64_t live, const TopScratch& s,
                      uint8_t* out_recs, uint32_t* slot_of_out, int sm_count, cudaStream_t st);
 
 // fa_lookup_flows (evict.cu): for each of the n 40-byte keys (device, 8-byte aligned) its slot in `t` or kNoSlot into
@@ -134,13 +157,10 @@ struct ExpireScratch {
     uint64_t cap;
     ExpireCtr* ctr;                                // zeroed before the mark
 };
-// Mark: the expire bitmap, the expiring slots (the first cap of them) and their count in s.ctr->n.  Reads only.
+// Mark: the expire bitmap, the expiring slots (the first cap of them) and their count in s.ctr->n.  Reads only.  Their
+// rows: launch_gather over s.list.
 int launch_expire_mark(const Table& t, uint64_t now, uint64_t idle, uint64_t active, const ExpireScratch& s, int sm_count,
                        cudaStream_t st);
-// Emit: rows of the n listed slots into out_recs (device, n x 144 B), their slots into slot_of_out (optional, for the
-// feature pass).  kmap: KERNEL_MAP record layout.
-int launch_expire_emit(const Table& t, bool kmap, const ExpireScratch& s, uint64_t n, uint8_t* out_recs, uint32_t* slot_of_out,
-                       int sm_count, cudaStream_t st);
 // Delete the n marked flows with every line they own, move the survivors of their clusters back towards their home slots,
 // and take n off ctr->live.  full: the table has no EMPTY slot (one thread, backward-shift deletion).
 int launch_expire_delete(const Table& t, const ExpireScratch& s, uint64_t n, bool full, Counters* ctr, int sm_count,

@@ -2,7 +2,7 @@
 
 Shapes: the headline sizing (ACCOUNTER, 2^25 slots, 2^26 device-generated records, tools/top_flows_bench.py's fill):
 10^6 and 10^7 Zipf-1.1 keys and 10^7 uniform keys, plus the 10^7 Zipf table of an engine with RTT and DNS folds where
-2^20 flows carry additional and DNS samples (row_times then reads feature lines too).  Per mask (all-zero: 1 group;
+2^20 flows carry additional and DNS samples (the row reader then reads feature lines too).  Per mask (all-zero: 1 group;
 proto + dst port: few; src /120: many; all-ones: one per flow) the call is warmed up, then timed --reps times with the host
 clock around it (it returns when its output is complete), output into device memory.  fa_top_flows(k = 10) is timed the
 same way as the cost of one existing full-table read-side scan.
