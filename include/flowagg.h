@@ -537,6 +537,43 @@ typedef struct fa_hist_row {     /* header of one row; n_bounds + 1 u64 bucket c
 int fa_histogram_flows(fa_engine* e, const uint8_t key_mask[40], uint32_t value, const uint64_t* bounds, uint32_t n_bounds,
                        void* out, size_t cap, size_t* n_groups);
 
+/* One group of fa_distinct_flows, 56 bytes. */
+typedef struct fa_distinct_group {
+    fa_flow_id key;                  /*  0 the group: a flow key AND group_mask (byte 39 = 0), as fa_flow_group.key */
+    uint64_t   flows;                /* 40 live flows in the group (feature-only flows included), as fa_flow_group.flows */
+    uint64_t   distinct;             /* 48 distinct values of (flow key AND distinct_mask) among those flows, >= 1 */
+} fa_distinct_group;
+
+/* Per-group distinct counts of a second key mask over the live flows (distinct destination ports per source: a port
+ * scan; distinct peers per host: fan-out; distinct clients per service: fan-in; distinct destinations of the window),
+ * on the device, WITHOUT removing or changing anything (no reference analogue: downstream of the agent the same COUNT
+ * DISTINCT runs on the host over evicted flows).
+ *   Group:  as fa_group_flows with key_mask = group_mask: the same groups, keys and flow counts.  `distinct` counts the
+ *           distinct 40-byte values key AND distinct_mask among the group's live flows.  Both masks are host memory, 40
+ *           bytes; byte 39 of each is ignored.  The masks may overlap: distinct_mask within group_mask gives 1 for every
+ *           group, an all-zero group_mask one row with the window's distinct count, an all-ones distinct_mask
+ *           distinct == flows.  Only the keys of the rows fa_evict_ex would return matter, in both modes (feature-only
+ *           flows included).
+ *   Threshold: only the groups with distinct >= min_distinct are returned (0 and 1: every group), so that a scan
+ *           detector is one call that returns a handful of rows.
+ *   Output: every passing group exactly once, in unspecified order, into `out` (host pageable / pinned or device
+ *           memory; device memory 8-byte aligned), room for cap rows.  *n_groups = the number of passing groups.
+ *   Nothing changes: the table, the feature lines, the live count, the sketch, the DNS correlation table, the fallback
+ *           ring and fa_group_flows' group table are as before, and a later eviction returns what it would have returned
+ *           without the call; in fa_stats only kernel_launches and d2h_bytes move.
+ *   Runs on the engine stream after every queued fold, under the engine lock, and returns when `out` is complete.
+ *   FA_F_NONBLOCKING_EVICT: counts the live table only, not a retired table still being evicted.  The fallback ring
+ *   (fa_read_spilled) is not part of the table.  Device scratch, allocated on first use and grown with the live count:
+ *   fa_group_flows' group table (it holds the distinct (group, value) pairs), a second group table of the same slot
+ *   layout sized from the number of those pairs, and 56 B per passing group of staging for a host `out`.
+ *   FA_E_2BIG: more than cap passing groups; *n_groups = the exact count and nothing is written to `out`.  `out` may be
+ *   NULL when cap == 0: a count query.
+ *   FA_E_INVAL: null engine / group_mask / distinct_mask / n_groups, out == NULL with cap > 0, device `out` not 8-byte
+ *   aligned (nothing changes).
+ *   FA_E_CUDA: a fold found no slot in a group table (never expected; the group tables are cleared all the same). */
+int fa_distinct_flows(fa_engine* e, const uint8_t group_mask[40], const uint8_t distinct_mask[40], uint64_t min_distinct,
+                      fa_distinct_group* out, size_t cap, size_t* n_groups);
+
 /* Lookup-and-RESET (no reference analogue; building block of the multi-GPU local combiner, the counterpart of
  * the reference folding its per-CPU maps in user space, pkg/tracer/tracer.go:1159-1187): every flow that received
  * records since the previous drain is written to out_records (device memory, cap x 144 B) as a partial flow record

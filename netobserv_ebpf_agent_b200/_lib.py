@@ -67,6 +67,10 @@ GROUP_DTYPE = np.dtype([("key", "u1", 40), ("flows", "<u8"), ("bytes", "<u8"), (
                         ("start_mono_time_ts", "<u8"), ("end_mono_time_ts", "<u8"), ("flags", "<u2"), ("pad_", "u1", 6)])
 assert GROUP_DTYPE.itemsize == 88
 
+# fa_distinct_group (56 bytes), include/flowagg.h
+DISTINCT_DTYPE = np.dtype([("key", "u1", 40), ("flows", "<u8"), ("distinct", "<u8")])
+assert DISTINCT_DTYPE.itemsize == 56
+
 
 def hist_dtype(n_bounds):
     """One row of fa_histogram_flows with n_bounds bounds: fa_hist_row, then n_bounds + 1 bucket counts
@@ -104,6 +108,8 @@ SIGNATURES = {
     "fa_group_flows": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_size_t, C.POINTER(C.c_size_t)]),
     "fa_histogram_flows": (C.c_int, [C.c_void_p, C.c_void_p, C.c_uint32, C.c_void_p, C.c_uint32, C.c_void_p, C.c_size_t,
                                      C.POINTER(C.c_size_t)]),
+    "fa_distinct_flows": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_uint64, C.c_void_p, C.c_size_t,
+                                    C.POINTER(C.c_size_t)]),
     "fa_evict": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_size_t,
                            C.POINTER(C.c_size_t)]),
     "fa_drain_active": (C.c_int, [C.c_void_p, C.c_void_p, C.c_size_t, C.POINTER(C.c_size_t)]),

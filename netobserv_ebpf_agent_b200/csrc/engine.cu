@@ -167,6 +167,10 @@ struct fa_engine {
     uint32_t* d_hist_row_of = nullptr;        // fa_histogram_flows, under `mu`: row of each group, one u32 per group-table slot
     uint8_t* d_hist_out = nullptr;            // ... and its staging of host-bound rows, hist_out_bytes
     uint64_t hist_out_bytes = 0;
+    fa::GroupScratch distinct{};              // fa_distinct_flows, under `mu`: the second group table (all zero between calls)
+    fa::GroupCtr* h_distinct_ctr = nullptr;   // pinned
+    uint8_t* d_distinct_out = nullptr;        // ... and its staging of host-bound rows, distinct_out_bytes
+    uint64_t distinct_out_bytes = 0;
     uint32_t* d_slot_of = nullptr;            // per-sample slot scratch of the feature folds
     uint64_t feat_seq[3] = {0, 0, 0};         // running sample numbers (additional, dns, packet drops)
     uint32_t* d_route_tmp = nullptr; unsigned long long* d_route_counts = nullptr;
@@ -708,6 +712,8 @@ void fa_destroy(fa_engine* e) {
     cudaFree(e->group.tab); cudaFree(e->group.list); cudaFree(e->group.ctr); cudaFree(e->d_group_out);
     if (e->h_group_ctr) cudaFreeHost(e->h_group_ctr);
     cudaFree(e->d_hist_row_of); cudaFree(e->d_hist_out);
+    cudaFree(e->distinct.tab); cudaFree(e->distinct.list); cudaFree(e->distinct.ctr); cudaFree(e->d_distinct_out);
+    if (e->h_distinct_ctr) cudaFreeHost(e->h_distinct_ctr);
     cudaFree(e->sk.cms); cudaFree(e->sk.hll);
     cudaFree(e->dnsc.tab); cudaFree(e->dnsc_spare); cudaFree(e->dnsc.ctr); cudaFreeHost(e->h_dnsc_ctr);
     cudaFree(e->d_dnsc_state); cudaFree(e->d_dnsc_samples); cudaFree(e->d_dnsc_out); cudaFree(e->d_dnsc_warps);
@@ -1269,22 +1275,32 @@ static int grow_group_out(uint8_t** buf, uint64_t* have_bytes, uint64_t n, uint6
     return FA_OK;
 }
 
-// The group table (all zero between calls), its list and counters for `live` flows, allocated on first use and grown
-// with the live count; with_row_of: also fa_histogram_flows' row index, one u32 per slot, grown with the table.
-static int grow_group_table(fa_engine* e, uint64_t live, bool with_row_of) {
-    uint64_t slots = 1024;                             // load factor <= 3/4: groups never outnumber the live flows
-    while (slots < (4 * live + 2) / 3) slots <<= 1;
-    if (!e->group.tab || e->group.mask + 1 < slots) {
-        cudaFree(e->group.tab); cudaFree(e->group.list); cudaFree(e->d_hist_row_of);
-        e->group.tab = nullptr; e->group.list = nullptr; e->group.mask = 0; e->d_hist_row_of = nullptr;
-        CU(cudaMalloc(&e->group.tab, slots * fa::kGroupSlotWords * 8));
-        CU(cudaMalloc(&e->group.list, slots * 4));
-        CU(cudaMemsetAsync(e->group.tab, 0, slots * fa::kGroupSlotWords * 8, e->stream));
-        e->group.mask = slots - 1;
+// A group table (all zero between calls), its list and counters for up to n groups, allocated on first use and grown
+// with n, and its pinned host counter.  *grown: the table was (re)allocated.
+static int grow_groups(fa::GroupScratch* g, fa::GroupCtr** h_ctr, uint64_t n, cudaStream_t st, bool* grown) {
+    uint64_t slots = 1024;                             // load factor <= 3/4: groups never outnumber n
+    while (slots < (4 * n + 2) / 3) slots <<= 1;
+    *grown = !g->tab || g->mask + 1 < slots;
+    if (*grown) {
+        cudaFree(g->tab); cudaFree(g->list);
+        g->tab = nullptr; g->list = nullptr; g->mask = 0;
+        CU(cudaMalloc(&g->tab, slots * fa::kGroupSlotWords * 8));
+        CU(cudaMalloc(&g->list, slots * 4));
+        CU(cudaMemsetAsync(g->tab, 0, slots * fa::kGroupSlotWords * 8, st));
+        g->mask = slots - 1;
     }
+    if (!g->ctr) CU(cudaMalloc(&g->ctr, sizeof(fa::GroupCtr)));
+    if (!*h_ctr) CU(cudaHostAlloc(h_ctr, sizeof(fa::GroupCtr), cudaHostAllocDefault));
+    return FA_OK;
+}
+
+// The group table of fa_group_flows for `live` flows; with_row_of: also fa_histogram_flows' row index, one u32 per slot,
+// grown with the table.
+static int grow_group_table(fa_engine* e, uint64_t live, bool with_row_of) {
+    bool grown = false;
+    if (int rc = grow_groups(&e->group, &e->h_group_ctr, live, e->stream, &grown)) return rc;
+    if (grown) { cudaFree(e->d_hist_row_of); e->d_hist_row_of = nullptr; }
     if (with_row_of && !e->d_hist_row_of) CU(cudaMalloc(&e->d_hist_row_of, (e->group.mask + 1) * 4));
-    if (!e->group.ctr) CU(cudaMalloc(&e->group.ctr, sizeof(fa::GroupCtr)));
-    if (!e->h_group_ctr) CU(cudaHostAlloc(&e->h_group_ctr, sizeof(fa::GroupCtr), cudaHostAllocDefault));
     return FA_OK;
 }
 
@@ -1425,6 +1441,91 @@ int fa_histogram_flows(fa_engine* e, const uint8_t key_mask[40], uint32_t value,
     e->st.d2h_bytes += d2h;
     if (rows && e->h_group_ctr->lost)
         rc = fail(FA_E_CUDA, "fa_histogram_flows: %llu flows did not find their group", e->h_group_ctr->lost);
+    if (rc == FA_OK || rc == FA_E_2BIG) *n_groups = (size_t)n;
+    return rc;
+}
+
+// Per-group distinct counts of a second key mask (evict.cu: launch_distinct_*), in two levels of the group table.  Level
+// 1 is the group scan with U = G | D (cap = live: never FA_E_2BIG): one group per distinct (key & G, key & D) pair,
+// because key & U is that pair and (key & U) & G == key & G.  Level 2 folds the listed pairs by & G into the second group
+// table (flows summed, pairs counted), then level 1 is cleared and its list, free again, receives the slots of the
+// level-2 groups that pass min_distinct; their count is the second wait.  Then their rows are written (device `out` in
+// place, host `out` through the distinct staging) and the second table is cleared, or only cleared (FA_E_2BIG, errors).
+// Both group tables are all zero again for the next call.  Nothing of the flow table or the counters is written.
+static_assert(sizeof(fa_distinct_group) == fa::kDistinctRowBytes && offsetof(fa_distinct_group, flows) == 40 &&
+              offsetof(fa_distinct_group, distinct) == 48, "fa_distinct_group ABI");
+
+int fa_distinct_flows(fa_engine* e, const uint8_t group_mask[40], const uint8_t distinct_mask[40], uint64_t min_distinct,
+                      fa_distinct_group* out, size_t cap, size_t* n_groups) {
+    if (n_groups) *n_groups = 0;
+    if (!e || !group_mask || !distinct_mask || !n_groups || (!out && cap))
+        return fail(FA_E_INVAL, "fa_distinct_flows: null argument");
+    std::lock_guard<std::mutex> lk(e->mu);
+    CU(cudaSetDevice(e->device));
+    const bool out_dev = out && classify(out) == PTR_DEVICE;
+    if (out_dev && (reinterpret_cast<uintptr_t>(out) & 7))
+        return fail(FA_E_INVAL, "fa_distinct_flows: device out must be 8-byte aligned");
+    if (int rc = sync_counters(e)) return rc;          // the queued folds finish; exact live count
+    const uint64_t live = e->live_known;
+    if (live == 0) return FA_OK;
+    cudaStream_t st = e->stream;
+    uint8_t u[fa::kKeyBytes];
+    for (int i = 0; i < fa::kKeyBytes; i++) u[i] = group_mask[i] | distinct_mask[i];
+    fa::GroupMask gm;
+    memcpy(gm.w, group_mask, fa::kKeyBytes);
+    gm.w[4] &= 0x00FFFFFFFFFFFFFFull;
+    GroupScan g;
+    if (int rc = scan_groups(e, "fa_distinct_flows", u, live, live, false, &g)) return rc;
+    const fa::GroupScratch s1 = e->group;
+    const uint64_t n1 = g.n;
+    uint64_t launched = g.launched;
+    int rc = g.rc;
+    bool grown = false;
+    if (rc == FA_OK && (rc = grow_groups(&e->distinct, &e->h_distinct_ctr, n1, st, &grown)) != FA_OK)
+        (void)cudaGetLastError();                      // no pending error: level 1 is still cleared below
+    const fa::GroupScratch s2 = e->distinct;
+    const bool second = rc == FA_OK;
+    if (second) {
+        CU(cudaMemsetAsync(s2.ctr, 0, sizeof(fa::GroupCtr), st));
+        launched += fa::launch_distinct_fold(s1, n1, gm, s2, e->sm_count, st);
+    }
+    launched += fa::launch_group_emit(s1, std::min<uint64_t>(n1, s1.mask + 1), nullptr, e->sm_count, st);   // clear level 1
+    if (second) {
+        CU(cudaMemsetAsync(s1.ctr, 0, sizeof(fa::GroupCtr), st));
+        launched += fa::launch_distinct_select(s2, n1, min_distinct, s1.list, &s1.ctr->n, e->sm_count, st);
+        CU(cudaMemcpyAsync(e->h_group_ctr, s1.ctr, sizeof(fa::GroupCtr), cudaMemcpyDeviceToHost, st));
+        CU(cudaMemcpyAsync(e->h_distinct_ctr, s2.ctr, sizeof(fa::GroupCtr), cudaMemcpyDeviceToHost, st));
+    }
+    CU(cudaGetLastError());
+    CU(cudaStreamSynchronize(st));
+    uint64_t n2 = 0, n = 0;                            // level-2 groups, passing groups
+    if (second) {
+        n2 = e->h_distinct_ctr->n;
+        n = e->h_group_ctr->n;
+        if (e->h_distinct_ctr->lost || n2 > n1 || n > n2)
+            rc = fail(FA_E_CUDA, "fa_distinct_flows: %llu groups of %llu pairs, %llu passing, %llu folds without a slot",
+                      (unsigned long long)n2, (unsigned long long)n1, (unsigned long long)n, e->h_distinct_ctr->lost);
+        else if (n > cap)
+            rc = fail(FA_E_2BIG, "fa_distinct_flows: capacity %zu < %llu groups", cap, (unsigned long long)n);
+    }
+    uint64_t* rows = nullptr;
+    if (rc == FA_OK && n) {
+        if (out_dev) rows = reinterpret_cast<uint64_t*>(out);
+        else if ((rc = grow_group_out(&e->d_distinct_out, &e->distinct_out_bytes, n, fa::kDistinctRowBytes, e->slots,
+                                      "fa_distinct_flows")) == FA_OK)
+            rows = reinterpret_cast<uint64_t*>(e->d_distinct_out);
+    }
+    if (rows) launched += fa::launch_distinct_emit(s2, s1.list, n, rows, e->sm_count, st);
+    if (second) launched += fa::launch_group_emit(s2, std::min<uint64_t>(n2, s2.mask + 1), nullptr, e->sm_count, st);   // clear level 2
+    CU(cudaGetLastError());
+    uint64_t d2h = 0;
+    if (rows && !out_dev) {
+        CU(cudaMemcpyAsync(out, rows, n * fa::kDistinctRowBytes, cudaMemcpyDeviceToHost, st));
+        d2h = n * fa::kDistinctRowBytes;
+    }
+    CU(cudaStreamSynchronize(st));
+    e->st.kernel_launches += launched;
+    e->st.d2h_bytes += d2h;
     if (rc == FA_OK || rc == FA_E_2BIG) *n_groups = (size_t)n;
     return rc;
 }

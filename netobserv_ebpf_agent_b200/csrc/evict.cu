@@ -673,6 +673,46 @@ __device__ __forceinline__ bool group_fold(const GroupScratch& s, const uint64_t
     return false;
 }
 
+// The peer set of this lane's key k: the lanes that have a key (have) and whose key equals it in every one of its ten
+// 32-bit words (distinct keys can share a premix).  Returns the set's lane mask (0 without a key); the set's leader (its
+// lowest lane) ends with v folded over the set.  Every lane of the warp calls it, converged.
+__device__ __forceinline__ uint32_t peer_reduce(const uint64_t k[5], bool have, GroupVals& v) {
+    const int lane = threadIdx.x & 31;
+    const uint32_t active = __ballot_sync(0xFFFFFFFFu, have);
+    uint32_t peers = active;
+#pragma unroll
+    for (int i = 0; i < 5; i++) {
+        peers &= __match_any_sync(0xFFFFFFFFu, (uint32_t)k[i]);
+        peers &= __match_any_sync(0xFFFFFFFFu, (uint32_t)(k[i] >> 32));
+    }
+    if (!have) peers = 0u;
+    const int np = __popc(peers);
+    if (__any_sync(0xFFFFFFFFu, np > 1)) {
+        if (__all_sync(0xFFFFFFFFu, !have || peers == active)) {
+            // one peer set holds every key of the round (a coarse mask): a butterfly over the warp
+            for (int d = 16; d > 0; d >>= 1) {
+                const uint64_t b = __shfl_sync(0xFFFFFFFFu, v.bytes, lane ^ d), p = __shfl_sync(0xFFFFFFFFu, v.packets, lane ^ d);
+                const uint64_t ns = __shfl_sync(0xFFFFFFFFu, v.nstart, lane ^ d), e = __shfl_sync(0xFFFFFFFFu, v.end, lane ^ d);
+                const uint32_t f = __shfl_sync(0xFFFFFFFFu, v.flags, lane ^ d);
+                v.bytes += b; v.packets += p; v.nstart = ns > v.nstart ? ns : v.nstart; v.end = e > v.end ? e : v.end; v.flags |= f;
+            }
+        } else {
+            // several sets: step q, every lane reads the q-th lane of its own set (the leader is lane 0 of it)
+            GroupVals a = v;
+            const int most = (int)__reduce_max_sync(0xFFFFFFFFu, (unsigned)np);
+            for (int q = 1; q < most; q++) {
+                const int src = q < np ? (int)__fns(peers, 0, q + 1) : lane;
+                const uint64_t b = __shfl_sync(0xFFFFFFFFu, v.bytes, src), p = __shfl_sync(0xFFFFFFFFu, v.packets, src);
+                const uint64_t ns = __shfl_sync(0xFFFFFFFFu, v.nstart, src), e = __shfl_sync(0xFFFFFFFFu, v.end, src);
+                const uint32_t f = __shfl_sync(0xFFFFFFFFu, v.flags, src);
+                if (q < np) { a.bytes += b; a.packets += p; a.nstart = ns > a.nstart ? ns : a.nstart; a.end = e > a.end ? e : a.end; a.flags |= f; }
+            }
+            v = a;
+        }
+    }
+    return peers;
+}
+
 __global__ void __launch_bounds__(256) group_scan_kernel(Table t, GroupMask m, GroupScratch s) {
     const int lane = threadIdx.x & 31;
     FOR_OCC_WORDS(t, w) {
@@ -690,38 +730,8 @@ __global__ void __launch_bounds__(256) group_scan_kernel(Table t, GroupMask m, G
                 const RowVals r = row_read(t, slot, true);
                 v = GroupVals{r.bytes, r.packets, 0ull - r.start, r.end, r.flags};
             }
-            const uint32_t active = __ballot_sync(0xFFFFFFFFu, have);
-            uint32_t peers = active;
-#pragma unroll
-            for (int i = 0; i < 5; i++) {
-                peers &= __match_any_sync(0xFFFFFFFFu, (uint32_t)k[i]);
-                peers &= __match_any_sync(0xFFFFFFFFu, (uint32_t)(k[i] >> 32));
-            }
-            if (!have) peers = 0u;
+            const uint32_t peers = peer_reduce(k, have, v);
             const int np = __popc(peers);
-            if (__any_sync(0xFFFFFFFFu, np > 1)) {
-                if (__all_sync(0xFFFFFFFFu, !have || peers == active)) {
-                    // one peer set holds every flow of the round (a coarse mask): a butterfly over the warp
-                    for (int d = 16; d > 0; d >>= 1) {
-                        const uint64_t b = __shfl_sync(0xFFFFFFFFu, v.bytes, lane ^ d), p = __shfl_sync(0xFFFFFFFFu, v.packets, lane ^ d);
-                        const uint64_t ns = __shfl_sync(0xFFFFFFFFu, v.nstart, lane ^ d), e = __shfl_sync(0xFFFFFFFFu, v.end, lane ^ d);
-                        const uint32_t f = __shfl_sync(0xFFFFFFFFu, v.flags, lane ^ d);
-                        v.bytes += b; v.packets += p; v.nstart = ns > v.nstart ? ns : v.nstart; v.end = e > v.end ? e : v.end; v.flags |= f;
-                    }
-                } else {
-                    // several sets: step q, every lane reads the q-th lane of its own set (the leader is lane 0 of it)
-                    GroupVals a = v;
-                    const int most = (int)__reduce_max_sync(0xFFFFFFFFu, (unsigned)np);
-                    for (int q = 1; q < most; q++) {
-                        const int src = q < np ? (int)__fns(peers, 0, q + 1) : lane;
-                        const uint64_t b = __shfl_sync(0xFFFFFFFFu, v.bytes, src), p = __shfl_sync(0xFFFFFFFFu, v.packets, src);
-                        const uint64_t ns = __shfl_sync(0xFFFFFFFFu, v.nstart, src), e = __shfl_sync(0xFFFFFFFFu, v.end, src);
-                        const uint32_t f = __shfl_sync(0xFFFFFFFFu, v.flags, src);
-                        if (q < np) { a.bytes += b; a.packets += p; a.nstart = ns > a.nstart ? ns : a.nstart; a.end = e > a.end ? e : a.end; a.flags |= f; }
-                    }
-                    v = a;
-                }
-            }
             if (have && lane == __ffs(peers) - 1 && !group_fold(s, k, (uint64_t)np, v)) atomicAdd(&s.ctr->lost, 1ull);
         }
     }
@@ -894,6 +904,86 @@ int launch_hist_emit(const GroupScratch& s, uint64_t n, uint32_t n_bounds, uint6
     if (!n) return 0;
     FA_LAUNCH(hist_emit_kernel, grid_for(n, sm_count), 256, 0, st, s, (unsigned long long)n, n_bounds,
               reinterpret_cast<unsigned long long*>(rows));
+    return 1;
+}
+
+// ---- fa_distinct_flows: per-group distinct counts of a second key mask, without removing or changing anything --------
+// Level 1 is launch_group_scan with U = G | D: its groups are the distinct (key & G, key & D) pairs, since both are
+// functions of key & U and key & U is their OR.  Level 2 takes the n1 listed level-1 groups, one per lane per round,
+// masks each key with G ((key & U) & G == key & G), forms peer sets as group_scan_kernel does and folds each set into
+// the second group table: the summed level-1 flow counts into flows (word 6), the set's size into word 7, which in the
+// second table holds the distinct count.  Every accumulator adds, so the result does not depend on the order.
+__global__ void __launch_bounds__(256) distinct_fold_kernel(GroupScratch s1, unsigned long long n1, GroupMask m, GroupScratch s2) {
+    const int lane = threadIdx.x & 31;
+    // warp-uniform steps (n1 is not a multiple of 32): every lane reaches the matches
+    for (unsigned long long i0 = blockIdx.x * (unsigned long long)blockDim.x + (threadIdx.x & ~31u); i0 < n1;
+         i0 += (unsigned long long)gridDim.x * blockDim.x) {
+        const unsigned long long i = i0 + lane;
+        const bool have = i < n1;
+        uint64_t k[5] = {0, 0, 0, 0, 0};
+        GroupVals v = {0, 0, 0, 0, 0u};                           // bytes carries the level-1 flow count
+        if (have) {
+            const unsigned long long* G = s1.tab + (uint64_t)s1.list[i] * kGroupSlotWords;
+#pragma unroll
+            for (int w = 0; w < 5; w++) k[w] = G[w] & m.w[w];
+            v.bytes = G[6];
+        }
+        const uint32_t peers = peer_reduce(k, have, v);
+        const int np = __popc(peers);
+        if (have && lane == __ffs(peers) - 1 && !group_fold(s2, k, v.bytes, GroupVals{(uint64_t)np, 0, 0, 0, 0u}))
+            atomicAdd(&s2.ctr->lost, 1ull);
+    }
+}
+
+// The slots of the level-2 groups with distinct >= min_distinct into sel, counted in *n_sel (zeroed before).  The group
+// count is read on the device; bound (>= it) sizes the grid.
+__global__ void __launch_bounds__(256) distinct_select_kernel(GroupScratch s2, unsigned long long min_distinct, uint32_t* __restrict__ sel,
+                                                              unsigned long long* n_sel) {
+    const unsigned long long n = s2.ctr->n;
+    const int lane = threadIdx.x & 31;
+    for (unsigned long long i0 = blockIdx.x * (unsigned long long)blockDim.x + (threadIdx.x & ~31u); i0 < n;
+         i0 += (unsigned long long)gridDim.x * blockDim.x) {
+        const unsigned long long i = i0 + lane;
+        uint32_t slot = 0;
+        bool take = false;
+        if (i < n) {
+            slot = s2.list[i];
+            take = s2.tab[(uint64_t)slot * kGroupSlotWords + 7] >= min_distinct;
+        }
+        const unsigned long long at = warp_reserve(take ? 1u : 0u, n_sel);
+        if (take) sel[at] = slot;
+    }
+}
+
+// Row i (fa_distinct_group: key, flows, distinct) from the level-2 group at slot sel[i].  The table is left as it is
+// (launch_group_emit with out == nullptr clears it).
+__global__ void __launch_bounds__(256) distinct_emit_kernel(GroupScratch s2, const uint32_t* __restrict__ sel, unsigned long long n,
+                                                            uint64_t* __restrict__ out) {
+    for (unsigned long long i = blockIdx.x * (unsigned long long)blockDim.x + threadIdx.x; i < n; i += (unsigned long long)gridDim.x * blockDim.x) {
+        const unsigned long long* G = s2.tab + (uint64_t)sel[i] * kGroupSlotWords;
+        uint64_t* O = out + i * (kDistinctRowBytes / 8);
+        for (int w = 0; w < 5; w++) O[w] = G[w];
+        O[5] = G[6]; O[6] = G[7];                               // flows, distinct
+    }
+}
+
+// One text for the device and the host emulation (FA_LAUNCH): every kernel loops grid-stride.
+int launch_distinct_fold(const GroupScratch& s1, uint64_t n1, const GroupMask& m, const GroupScratch& s2, int sm_count, cudaStream_t st) {
+    if (!n1) return 0;
+    FA_LAUNCH(distinct_fold_kernel, grid_for(n1, sm_count), 256, 0, st, s1, (unsigned long long)n1, m, s2);
+    return 1;
+}
+
+int launch_distinct_select(const GroupScratch& s2, uint64_t bound, uint64_t min_distinct, uint32_t* sel, unsigned long long* n_sel,
+                           int sm_count, cudaStream_t st) {
+    if (!bound) return 0;
+    FA_LAUNCH(distinct_select_kernel, grid_for(bound, sm_count), 256, 0, st, s2, (unsigned long long)min_distinct, sel, n_sel);
+    return 1;
+}
+
+int launch_distinct_emit(const GroupScratch& s2, const uint32_t* sel, uint64_t n, uint64_t* out, int sm_count, cudaStream_t st) {
+    if (!n) return 0;
+    FA_LAUNCH(distinct_emit_kernel, grid_for(n, sm_count), 256, 0, st, s2, sel, (unsigned long long)n, out);
     return 1;
 }
 

@@ -204,6 +204,18 @@ int launch_hist_scan(const Table& t, const GroupMask& m, const GroupScratch& s, 
 // (launch_group_emit with out == nullptr clears it).
 int launch_hist_emit(const GroupScratch& s, uint64_t n, uint32_t n_bounds, uint64_t* rows, int sm_count, cudaStream_t st);
 
+// fa_distinct_flows (evict.cu): a second level over the groups that launch_group_scan built with G | D (key & (G | D) is
+// one (key & G, key & D) pair), folded by key & G into a second group table whose word 7 holds the distinct count.
+constexpr int kDistinctRowBytes = 56;              // one fa_distinct_group row
+// Fold the n1 listed groups of s1 into s2 (all zero before, its counters zeroed) by their key AND m.  Reads s1 only.
+int launch_distinct_fold(const GroupScratch& s1, uint64_t n1, const GroupMask& m, const GroupScratch& s2, int sm_count, cudaStream_t st);
+// The slots of s2's groups with distinct >= min_distinct into sel, their number into *n_sel (zeroed before).  bound: at
+// least s2's group count (the grid).  Reads s2 only.
+int launch_distinct_select(const GroupScratch& s2, uint64_t bound, uint64_t min_distinct, uint32_t* sel, unsigned long long* n_sel,
+                           int sm_count, cudaStream_t st);
+// Rows of the n groups at slots sel[i] of s2 as fa_distinct_group into out (device, 8-byte aligned).  s2 is left as it is.
+int launch_distinct_emit(const GroupScratch& s2, const uint32_t* sel, uint64_t n, uint64_t* out, int sm_count, cudaStream_t st);
+
 // sketches
 int launch_cms_query(const SketchParams& sk, const uint4* keys, uint32_t n, unsigned long long* est, cudaStream_t st);
 int launch_hll_pack(const SketchParams& sk, uint8_t* out_regs, cudaStream_t st);

@@ -275,6 +275,23 @@ class FlowAggEngine:
                                        C.byref(got)))
         return out[: got.value]
 
+    def distinct_flows(self, group_mask, distinct_mask, min_distinct=0, cap=None):
+        """Per-group distinct counts over the live flows, without changing anything -> a DISTINCT_DTYPE array, one row
+        per group of the 40-byte key mask group_mask (as group_flows) with at least min_distinct distinct values of
+        key & distinct_mask (both masks from group_mask()), in unspecified order.  cap: room in groups (default: the live
+        count right now)."""
+        from ._lib import DISTINCT_DTYPE
+        g = np.ascontiguousarray(group_mask, dtype=np.uint8).reshape(-1)
+        d = np.ascontiguousarray(distinct_mask, dtype=np.uint8).reshape(-1)
+        assert g.size == 40 and d.size == 40, (g.size, d.size)
+        if cap is None:
+            cap = max(self.live_flows(), 1)
+        out = np.zeros(cap, DISTINCT_DTYPE)
+        got = C.c_size_t(0)
+        check(lib().fa_distinct_flows(self._h, g.ctypes.data, d.ctypes.data, int(min_distinct), out.ctypes.data, cap,
+                                      C.byref(got)))
+        return out[: got.value]
+
     def read_spilled(self, cap=131072):
         """KERNEL_MAP mode with FA_F_RINGBUF_FALLBACK: the single-packet records that could not enter the full map
         (the batched equivalent of reading the direct_flows ring buffer) -> (n,144) uint8 array."""
