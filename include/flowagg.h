@@ -705,22 +705,73 @@ int fa_route_peer(fa_engine* e, const void* records_dev, const uint64_t* n_dev, 
  * their owners over NVLink (fa_route_peer) and folds what it receives; the only synchronisation is device-side
  * (events between the N streams).  cfg: mode ACCOUNTER; max_entries = flows of the whole box; max_batch = records per
  * GPU and round (0 = 2^22); reserved0 bit 0 = route raw records (no local combiner); device / cuda_stream ignored.
- * fa_sharded_evict == LookupAndDeleteMap over all owners (disjoint key sets, concatenated). */
+ * flags: FA_F_ENABLE_RTT / _DNS / _PKT_DROP are passed to the owners (the combiners do not get them: samples bypass
+ * the combiner); FA_F_ENABLE_SKETCH is refused (FA_E_INVAL).  A device id may appear more than once: several shards
+ * then share one GPU (peer access is only enabled between distinct devices).
+ * fa_sharded_evict == LookupAndDeleteMap over all owners (disjoint key sets, concatenated).
+ * All calls take the object's lock: one thread at a time, calls of several threads are serialised. */
 typedef struct fa_sharded fa_sharded;
 int  fa_sharded_create(const fa_config* cfg, const int32_t* devices, uint32_t n_devices, fa_sharded** out);
 void fa_sharded_destroy(fa_sharded* s);
 int  fa_sharded_ingest(fa_sharded* s, const void* flow_records_host, size_t n);
 /* device-resident batches: records_dev[i] (n_per_gpu[i] records) lives on devices[i] */
 int  fa_sharded_ingest_device(fa_sharded* s, const void* const* records_dev, const size_t* n_per_gpu);
+/* Feature samples, host memory (pageable or pinned, released before return, as fa_sharded_ingest): n (flow_id +
+ * additional_metrics), (flow_id + dns_metrics) or (flow_id + pkt_drop_metrics) samples, folded on the GPU that owns their
+ * flow.  A call is cut into rounds of at most N x max_batch samples; slice i of a round goes to GPU i, which routes it
+ * stably (fa_route_peer_samples) into its segment of every owner's receive buffer; each owner folds the segments in
+ * source order (fa_ingest_samples_counted), so every owner folds a flow's samples in stream order.
+ * Exactness: for any sequence of fa_sharded_ingest / _additional / _dns / _pkt_drops calls, fa_sharded_evict_ex returns,
+ * sorted by key, the rows one engine with the same flags returns for the same calls in the same order, bit for bit in the
+ * dns, additional, pkt_drops, rtt_min and present blocks and in the base patch of feature-only flows, for arbitrary
+ * sample values.  The 144-byte base rows themselves are exact under fa_sharded_ingest's condition (per-flow-constant
+ * descriptors).  Sample and record calls share the rounds and stay ordered on every GPU.  Counted in fa_sharded_get_stats'
+ * additional / dns / pkt_drops_ingested.  FA_E_INVAL: the object was created without the kind's FA_F_ENABLE_* flag,
+ * null samples with n > 0, device memory (device-resident samples are not supported).  Not available: K7's
+ * fa_ingest_dns_packets (a query and its response have reversed tuples, hence different owners), sketches, KERNEL_MAP. */
+int  fa_sharded_ingest_additional(fa_sharded* s, const void* additional_records_host, size_t n);
+int  fa_sharded_ingest_dns(fa_sharded* s, const void* dns_records_host, size_t n);
+int  fa_sharded_ingest_pkt_drops(fa_sharded* s, const void* pkt_drop_records_host, size_t n);
 int  fa_sharded_evict(fa_sharded* s, void* out_records_host, size_t cap, size_t* n_out);
+/* fa_evict_ex over all owners: the blocks of `out` as in fa_evict_ex (host memory; `records` required when flows are
+ * live, the others may be NULL), each with room for cap rows; the owners' rows are concatenated (disjoint key sets),
+ * order unspecified.  The combiners' scratch tables are emptied as by fa_sharded_evict (which is this call with records
+ * only).  FA_E_2BIG (nothing evicted): cap < live flows; FA_E_INVAL: null argument or records. */
+int  fa_sharded_evict_ex(fa_sharded* s, const fa_evict_out* out, size_t cap, size_t* n_out);
 int  fa_sharded_live_flows(fa_sharded* s, size_t* n);
 int  fa_sharded_sync(fa_sharded* s);
-/* sum of the owners' counters; nvlink_records = records that crossed to another GPU; receive_overflow must stay 0 */
+/* sum of the owners' counters (records_ingested and the three sample counts: what was passed in); nvlink_records =
+ * 144-byte records that crossed to another GPU (samples are not counted there); receive_overflow must stay 0 */
 int  fa_sharded_get_stats(fa_sharded* s, fa_stats* sum, uint64_t* nvlink_records, uint64_t* receive_overflow);
 const char* fa_sharded_last_error(void);
 /* fa_ingest for a device-resident batch whose size (<= max_n) is only known on the device; reset_count != 0
  * zeroes *n_dev after the fold has been enqueued.  Requires FA_F_NO_FULL_CUT. */
 int fa_ingest_counted(fa_engine* e, const void* records_dev, uint64_t* n_dev, size_t max_n, int reset_count);
+
+/* ---- the exchange for feature samples (what fa_sharded_ingest_additional / _dns / _pkt_drops run on) ----
+ * kind: which sample stream, as fa_ingest_additional (72 B), fa_ingest_dns (104 B) and fa_ingest_pkt_drops (72 B). */
+enum fa_sample_kind { FA_SAMPLES_ADDITIONAL = 0, FA_SAMPLES_DNS = 1, FA_SAMPLES_PKT_DROPS = 2 };
+
+/* Route min(*n_dev, max_n) device-resident samples of `kind` (n_dev may be NULL: exactly max_n) to their owners, STABLY:
+ * the samples bound for owner o = fa_owner_hash(key) % n_shards (the owner of the flow's base records) are stored into
+ * peer_segs[o], this source's segment of o's receive buffer, in the order they have in `samples_dev`, and their number
+ * is stored (not added) into *peer_seg_counts[o].  Each segment holds seg_cap samples; seg_cap >= max_n cannot
+ * overflow.  A sample past the end is not stored and adds 1 to overflow_dev[0] (as does *n_dev - max_n when *n_dev >
+ * max_n); overflow_dev[1] is not touched (fa_route_peer counts 144-byte rows there).  Three kernels on the engine's
+ * stream, no host synchronisation; the engine's flags do not matter.  Samples and segments 8-byte aligned, device (or
+ * peer-mapped) memory.  FA_E_INVAL: null argument, kind, n_shards not 1..16 or self_shard >= n_shards, alignment. */
+int fa_route_peer_samples(fa_engine* e, uint32_t kind, const void* samples_dev, const uint64_t* n_dev, size_t max_n, uint32_t n_shards,
+                          uint32_t self_shard, void* const* peer_segs, uint64_t* const* peer_seg_counts, size_t seg_cap, uint64_t* overflow_dev);
+
+/* Fold min(*n_dev, max_n) device-resident samples of `kind` whose count lives in device memory (one segment of a receive
+ * buffer), as fa_ingest_additional / _dns / _pkt_drops would fold them: the samples get the engine's next max_n sample
+ * numbers, so segments folded one after the other are folded in that order, bit-exactly (the unused numbers of a short
+ * segment are a gap; only the relative order of a flow's samples matters).  reset_count != 0 zeroes *n_dev after the fold
+ * has been enqueued.  Asynchronous on the engine's stream; the samples must stay valid until it has run.  Not counted in
+ * fa_stats' additional / dns / pkt_drops_ingested (the count is not known on the host).  A sample whose flow cannot be
+ * created counts in `spills`; there is no room check.  FA_E_INVAL: null argument, kind, engine without the kind's
+ * FA_F_ENABLE_* flag or without FA_F_NO_FULL_CUT, KERNEL_MAP mode, max_n not 1..max_batch, samples not 8-byte aligned. */
+int fa_ingest_samples_counted(fa_engine* e, uint32_t kind, const void* samples_dev, uint64_t* n_dev, size_t max_n, int reset_count);
 
 /* ------------------------------------------- memory + synthetic generator */
 

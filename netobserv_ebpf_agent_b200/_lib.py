@@ -16,6 +16,7 @@ FA_TOP_BYTES, FA_TOP_PACKETS, FA_TOP_MAX_K = 0, 1, 1 << 20
 FA_HIST_BYTES, FA_HIST_PACKETS, FA_HIST_DURATION, FA_HIST_RTT, FA_HIST_DNS_LATENCY = 0, 1, 2, 3, 4
 FA_HIST_MAX_BOUNDS = 63
 FA_GEN_UNIFORM, FA_GEN_ZIPF = 0, 1
+FA_SAMPLES_ADDITIONAL, FA_SAMPLES_DNS, FA_SAMPLES_PKT_DROPS = 0, 1, 2
 FA_ABI_VERSION = 1
 
 
@@ -120,12 +121,19 @@ SIGNATURES = {
     "fa_sharded_destroy": (None, [C.c_void_p]),
     "fa_sharded_ingest": (C.c_int, [C.c_void_p, C.c_void_p, C.c_size_t]),
     "fa_sharded_ingest_device": (C.c_int, [C.c_void_p, C.POINTER(C.c_void_p), C.POINTER(C.c_size_t)]),
+    "fa_sharded_ingest_additional": (C.c_int, [C.c_void_p, C.c_void_p, C.c_size_t]),
+    "fa_sharded_ingest_dns": (C.c_int, [C.c_void_p, C.c_void_p, C.c_size_t]),
+    "fa_sharded_ingest_pkt_drops": (C.c_int, [C.c_void_p, C.c_void_p, C.c_size_t]),
     "fa_sharded_evict": (C.c_int, [C.c_void_p, C.c_void_p, C.c_size_t, C.POINTER(C.c_size_t)]),
+    "fa_sharded_evict_ex": (C.c_int, [C.c_void_p, C.POINTER(EvictOut), C.c_size_t, C.POINTER(C.c_size_t)]),
     "fa_sharded_live_flows": (C.c_int, [C.c_void_p, C.POINTER(C.c_size_t)]),
     "fa_sharded_sync": (C.c_int, [C.c_void_p]),
     "fa_sharded_get_stats": (C.c_int, [C.c_void_p, C.POINTER(Stats), C.POINTER(C.c_uint64), C.POINTER(C.c_uint64)]),
     "fa_sharded_last_error": (C.c_char_p, []),
     "fa_ingest_counted": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_size_t, C.c_int]),
+    "fa_route_peer_samples": (C.c_int, [C.c_void_p, C.c_uint32, C.c_void_p, C.c_void_p, C.c_size_t, C.c_uint32, C.c_uint32,
+                                        C.POINTER(C.c_void_p), C.POINTER(C.c_void_p), C.c_size_t, C.c_void_p]),
+    "fa_ingest_samples_counted": (C.c_int, [C.c_void_p, C.c_uint32, C.c_void_p, C.c_void_p, C.c_size_t, C.c_int]),
     "fa_ipc_export": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p]),
     "fa_ipc_open": (C.c_int, [C.c_void_p, C.c_void_p, C.POINTER(C.c_void_p)]),
     "fa_ipc_close": (C.c_int, [C.c_void_p, C.c_void_p]),

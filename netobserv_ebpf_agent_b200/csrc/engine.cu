@@ -174,6 +174,8 @@ struct fa_engine {
     uint32_t* d_slot_of = nullptr;            // per-sample slot scratch of the feature folds
     uint64_t feat_seq[3] = {0, 0, 0};         // running sample numbers (additional, dns, packet drops)
     uint32_t* d_route_tmp = nullptr; unsigned long long* d_route_counts = nullptr;
+    uint32_t* d_sroute_hist = nullptr; uint64_t sroute_tiles = 0;   // fa_route_peer_samples: per-(owner, tile) counts ...
+    unsigned long long* d_sroute_tot = nullptr;                    // ... and per-owner totals
 
     fa::SketchParams sk{};
     unsigned long long* d_prof = nullptr;     // FA_PHASE_PROFILE=1: per-phase warp-cycle counters of K1
@@ -702,6 +704,7 @@ void fa_destroy(fa_engine* e) {
     cudaFree(e->d_scratch); cudaFree(e->d_spill_idx); cudaFree(e->d_cut_set); cudaFree(e->d_cut_bitmap); cudaFree(e->d_cut_out);
     if (e->h_cut_out) cudaFreeHost(e->h_cut_out);
     cudaFree(e->d_route_tmp); cudaFree(e->d_route_counts); cudaFree(e->d_expanded);
+    cudaFree(e->d_sroute_hist); cudaFree(e->d_sroute_tot);
     cudaFree(e->d_snap_src); cudaFree(e->d_snap_cnt); cudaFree(e->d_snap_verdict);
     free_staging(&e->evict_stage); free_staging(&e->top_stage); cudaFree(e->d_slot_of);
     cudaFree(e->top.state); cudaFree(e->top.hist); cudaFree(e->top.ents); if (e->h_top_state) cudaFreeHost(e->h_top_state);
@@ -1597,6 +1600,61 @@ int fa_ingest_counted(fa_engine* e, const void* recs, uint64_t* n_dev, size_t ma
     int rc = launch_chunk(e, static_cast<const uint8_t*>(recs), (uint32_t)max_n);
     e->k1_opt = saved;
     if (rc) return rc;
+    if (reset_count) CU(cudaMemsetAsync(n_dev, 0, 8, e->stream));
+    return FA_OK;
+}
+
+static const char* sample_kind_name(uint32_t kind) { return kind == 0 ? "FA_F_ENABLE_RTT" : kind == 1 ? "FA_F_ENABLE_DNS" : "FA_F_ENABLE_PKT_DROP"; }
+static uint32_t sample_kind_flag(uint32_t kind) { return kind == 0 ? FA_F_ENABLE_RTT : kind == 1 ? FA_F_ENABLE_DNS : FA_F_ENABLE_PKT_DROP; }
+
+int fa_route_peer_samples(fa_engine* e, uint32_t kind, const void* samples_dev, const uint64_t* n_dev, size_t max_n, uint32_t n_shards,
+                          uint32_t self_shard, void* const* peer_segs, uint64_t* const* peer_seg_counts, size_t seg_cap, uint64_t* overflow_dev) {
+    if (!e || !samples_dev || !peer_segs || !peer_seg_counts || !overflow_dev) return fail(FA_E_INVAL, "fa_route_peer_samples: null argument");
+    if (kind > FA_SAMPLES_PKT_DROPS) return fail(FA_E_INVAL, "fa_route_peer_samples: unknown sample kind %u", kind);
+    if (n_shards == 0 || n_shards > 16 || self_shard >= n_shards) return fail(FA_E_INVAL, "fa_route_peer_samples: n_shards must be 1..16, self_shard below it");
+    if (max_n > 0xFFFFFFFFull) return fail(FA_E_INVAL, "fa_route_peer_samples: max_n too large");
+    if (reinterpret_cast<uintptr_t>(samples_dev) & 7) return fail(FA_E_INVAL, "fa_route_peer_samples: samples must be 8-byte aligned");
+    for (uint32_t i = 0; i < n_shards; i++)
+        if (!peer_segs[i] || !peer_seg_counts[i] || (reinterpret_cast<uintptr_t>(peer_segs[i]) & 7))
+            return fail(FA_E_INVAL, "fa_route_peer_samples: segment %u missing or not 8-byte aligned", i);
+    std::lock_guard<std::mutex> lk(e->mu);
+    CU(cudaSetDevice(e->device));
+    const uint64_t tiles = (max_n + 255) / 256;
+    if (tiles > e->sroute_tiles) {                                   // scratch of the count pass, grown on demand
+        CU(cudaFree(e->d_sroute_hist)); e->d_sroute_hist = nullptr; e->sroute_tiles = 0;
+        CU(cudaMalloc(&e->d_sroute_hist, tiles * 16 * 4));
+        e->sroute_tiles = tiles;
+        if (!e->d_sroute_tot) CU(cudaMalloc(&e->d_sroute_tot, 16 * 8));
+    }
+    fa::PeerTargets pt{};
+    for (uint32_t i = 0; i < n_shards; i++) {
+        pt.buf[i] = static_cast<uint4*>(peer_segs[i]);
+        pt.count[i] = reinterpret_cast<unsigned long long*>(peer_seg_counts[i]);
+    }
+    e->st.kernel_launches += fa::launch_route_samples((int)kind, static_cast<const uint8_t*>(samples_dev), reinterpret_cast<const unsigned long long*>(n_dev),
+                                                      (uint32_t)max_n, n_shards, pt, seg_cap, e->d_sroute_hist, e->d_sroute_tot,
+                                                      reinterpret_cast<unsigned long long*>(overflow_dev), e->sm_count, e->stream);
+    CU(cudaGetLastError());
+    return FA_OK;
+}
+
+int fa_ingest_samples_counted(fa_engine* e, uint32_t kind, const void* samples_dev, uint64_t* n_dev, size_t max_n, int reset_count) {
+    if (!e || !samples_dev || !n_dev) return fail(FA_E_INVAL, "fa_ingest_samples_counted: null argument");
+    if (kind > FA_SAMPLES_PKT_DROPS) return fail(FA_E_INVAL, "fa_ingest_samples_counted: unknown sample kind %u", kind);
+    if (!(e->cfg.flags & sample_kind_flag(kind))) return fail(FA_E_INVAL, "fa_ingest_samples_counted: engine was created without %s", sample_kind_name(kind));
+    if (!(e->cfg.flags & FA_F_NO_FULL_CUT)) return fail(FA_E_INVAL, "fa_ingest_samples_counted: engine needs FA_F_NO_FULL_CUT");
+    if (e->cfg.mode != FA_MODE_ACCOUNTER) return fail(FA_E_INVAL, "fa_ingest_samples_counted: ACCOUNTER mode only");
+    if (max_n == 0 || max_n > e->max_batch) return fail(FA_E_INVAL, "fa_ingest_samples_counted: max_n must be 1..max_batch");
+    if (reinterpret_cast<uintptr_t>(samples_dev) & 7) return fail(FA_E_INVAL, "fa_ingest_samples_counted: samples must be 8-byte aligned");
+    std::lock_guard<std::mutex> lk(e->mu);
+    CU(cudaSetDevice(e->device));
+    // sample numbers feat_seq .. feat_seq + max_n - 1 are reserved for this segment; the unused ones are a harmless gap
+    e->st.kernel_launches += fa::launch_feature_fold_counted((int)kind, static_cast<const uint8_t*>(samples_dev), reinterpret_cast<const unsigned long long*>(n_dev),
+                                                             (uint32_t)max_n, e->table, ++e->epoch, e->feat_seq[kind], e->d_slot_of,
+                                                             e->d_ctr, e->sm_count, e->stream);
+    CU(cudaGetLastError());
+    e->feat_seq[kind] += max_n;
+    e->unsynced_records += max_n;
     if (reset_count) CU(cudaMemsetAsync(n_dev, 0, 8, e->stream));
     return FA_OK;
 }

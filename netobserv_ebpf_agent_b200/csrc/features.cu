@@ -216,10 +216,13 @@ template <class F> constexpr size_t feature_fold_smem() {
     return tile + kFeatRep * 4 + kFeatTile * 4 + kFeatTile * 4 + kFeatHot * sizeof(FeatHot<F>);
 }
 
-template <class F>
+// kDevN: the sample count is min(*n_dev, max_n), read from device memory (a count another GPU's route stored); the grid
+// is sized from max_n and the CTAs past the count only start and stop.  Otherwise n_dev is unused and n = max_n.
+template <class F, bool kDevN = false>
 __global__ void __launch_bounds__(kFeatTile, FA_K6_MINBLOCKS)
-feature_fold_kernel(const uint8_t* __restrict__ recs, uint32_t n, Table t, uint64_t epoch, uint64_t seq0,
-                    uint32_t* __restrict__ slot_of, Counters* ctr) {
+feature_fold_kernel(const uint8_t* __restrict__ recs, uint32_t max_n, Table t, uint64_t epoch, uint64_t seq0,
+                    uint32_t* __restrict__ slot_of, Counters* ctr, const unsigned long long* __restrict__ n_dev = nullptr) {
+    const uint32_t n = kDevN ? (uint32_t)min((unsigned long long)max_n, *n_dev) : max_n;
     FA_DYN_SMEM(sm);
     constexpr size_t kTileBytes = (size_t)kFeatTile * (F::kRec > F::kAcc * 8 ? F::kRec : F::kAcc * 8);
     uint64_t* tile = reinterpret_cast<uint64_t*>(sm);                         // kFeatTile samples ...
@@ -322,8 +325,10 @@ feature_fold_kernel(const uint8_t* __restrict__ recs, uint32_t n, Table t, uint6
 }
 
 // second pass: the sample that turned out to be the flow's first one writes the adopted block fields
-__global__ void additional_first_kernel(const uint8_t* __restrict__ recs, uint32_t n, Table t, uint64_t seq0,
-                                        const uint32_t* __restrict__ slot_of) {
+template <bool kDevN = false>
+__global__ void additional_first_kernel(const uint8_t* __restrict__ recs, uint32_t max_n, Table t, uint64_t seq0,
+                                        const uint32_t* __restrict__ slot_of, const unsigned long long* __restrict__ n_dev = nullptr) {
+    const uint32_t n = kDevN ? (uint32_t)min((unsigned long long)max_n, *n_dev) : max_n;
     for (uint32_t i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += gridDim.x * blockDim.x) {
         const uint32_t slot = slot_of[i];
         if (slot == 0xFFFFFFFFu) continue;
@@ -336,8 +341,10 @@ __global__ void additional_first_kernel(const uint8_t* __restrict__ recs, uint32
     }
 }
 
-__global__ void dns_first_kernel(const uint8_t* __restrict__ recs, uint32_t n, Table t, uint64_t seq0,
-                                 const uint32_t* __restrict__ slot_of) {
+template <bool kDevN = false>
+__global__ void dns_first_kernel(const uint8_t* __restrict__ recs, uint32_t max_n, Table t, uint64_t seq0,
+                                 const uint32_t* __restrict__ slot_of, const unsigned long long* __restrict__ n_dev = nullptr) {
+    const uint32_t n = kDevN ? (uint32_t)min((unsigned long long)max_n, *n_dev) : max_n;
     for (uint32_t i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += gridDim.x * blockDim.x) {
         const uint32_t slot = slot_of[i];
         if (slot == 0xFFFFFFFFu) continue;
@@ -351,8 +358,10 @@ __global__ void dns_first_kernel(const uint8_t* __restrict__ recs, uint32_t n, T
     }
 }
 
-__global__ void pktdrop_first_kernel(const uint8_t* __restrict__ recs, uint32_t n, Table t, uint64_t seq0,
-                                     const uint32_t* __restrict__ slot_of) {
+template <bool kDevN = false>
+__global__ void pktdrop_first_kernel(const uint8_t* __restrict__ recs, uint32_t max_n, Table t, uint64_t seq0,
+                                     const uint32_t* __restrict__ slot_of, const unsigned long long* __restrict__ n_dev = nullptr) {
+    const uint32_t n = kDevN ? (uint32_t)min((unsigned long long)max_n, *n_dev) : max_n;
     for (uint32_t i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += gridDim.x * blockDim.x) {
         const uint32_t slot = slot_of[i];
         if (slot == 0xFFFFFFFFu) continue;
@@ -369,31 +378,54 @@ __global__ void pktdrop_first_kernel(const uint8_t* __restrict__ recs, uint32_t 
     }
 }
 
+// persistent over tiles: exactly as many CTAs as are resident at once (a partial second wave would leave SMs idle)
+template <class F, bool kDevN>
+static uint32_t fold_grid(uint32_t n_tiles, int sm_count) {
 #ifndef FA_HOST_EMUL
-template <class F, class First>
-static int launch_fold(First first_kernel, const uint8_t* recs, uint32_t n, const Table& t, uint64_t epoch, uint64_t seq0, uint32_t* slot_of,
-                       Counters* ctr, int sm_count, cudaStream_t st) {
-    const uint32_t n_tiles = (n + kFeatTile - 1) / kFeatTile;
-    // persistent over tiles: exactly as many CTAs as are resident at once (a partial second wave would leave SMs idle)
     static int per_sm = 0;
     if (!per_sm) {
-        if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, feature_fold_kernel<F>, kFeatTile, feature_fold_smem<F>()) != cudaSuccess || per_sm < 1) per_sm = 4;
+        if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, feature_fold_kernel<F, kDevN>, kFeatTile, feature_fold_smem<F>()) != cudaSuccess || per_sm < 1) per_sm = 4;
     }
-    const uint32_t grid = std::min<uint32_t>(n_tiles, (uint32_t)(sm_count * per_sm));
-    feature_fold_kernel<F><<<grid, kFeatTile, feature_fold_smem<F>(), st>>>(recs, n, t, epoch, seq0, slot_of, ctr);
-    first_kernel<<<sm_count * 8, 256, 0, st>>>(recs, n, t, seq0, slot_of);
+    return std::min<uint32_t>(n_tiles, (uint32_t)(sm_count * per_sm));
+#else
+    (void)sm_count;
+    return n_tiles;
+#endif
+}
+
+// The fold and its second pass, for a host count (n = max_n) or a device one (min(*n_dev, max_n)); the same launches
+// either way, sized from max_n.
+using FirstKernel = void (*)(const uint8_t*, uint32_t, Table, uint64_t, const uint32_t*, const unsigned long long*);
+template <class F, bool kDevN>
+static int launch_fold(FirstKernel first_kernel, const uint8_t* recs, uint32_t max_n, const unsigned long long* n_dev, const Table& t,
+                       uint64_t epoch, uint64_t seq0, uint32_t* slot_of, Counters* ctr, int sm_count, cudaStream_t st) {
+    const uint32_t n_tiles = (max_n + kFeatTile - 1) / kFeatTile;
+    const auto fold = feature_fold_kernel<F, kDevN>;
+    const uint32_t grid = fold_grid<F, kDevN>(n_tiles, sm_count);
+    FA_LAUNCH(fold, grid, kFeatTile, feature_fold_smem<F>(), st, recs, max_n, t, epoch, seq0, slot_of, ctr, n_dev);
+    FA_LAUNCH(first_kernel, sm_count * 8, 256, 0, st, recs, max_n, t, seq0, slot_of, n_dev);
     return 2;
 }
 
+#ifndef FA_HOST_EMUL
 int launch_feature_fold(int kind, const uint8_t* recs, uint32_t n, const Table& t, uint64_t epoch, uint64_t seq0,
                         uint32_t* slot_of, Counters* ctr, int sm_count, cudaStream_t st) {
     if (!n) return 0;
     static_assert(feature_fold_smem<DnsFeat>() <= 48 * 1024 && feature_fold_smem<DropFeat>() <= 48 * 1024, "K6 tiles fit the default 48 KB");
-    if (kind == 2) return launch_fold<DropFeat>(pktdrop_first_kernel, recs, n, t, epoch, seq0, slot_of, ctr, sm_count, st);
-    if (kind == 0) return launch_fold<AddFeat>(additional_first_kernel, recs, n, t, epoch, seq0, slot_of, ctr, sm_count, st);
-    return launch_fold<DnsFeat>(dns_first_kernel, recs, n, t, epoch, seq0, slot_of, ctr, sm_count, st);
+    if (kind == 2) return launch_fold<DropFeat, false>(pktdrop_first_kernel<false>, recs, n, nullptr, t, epoch, seq0, slot_of, ctr, sm_count, st);
+    if (kind == 0) return launch_fold<AddFeat, false>(additional_first_kernel<false>, recs, n, nullptr, t, epoch, seq0, slot_of, ctr, sm_count, st);
+    return launch_fold<DnsFeat, false>(dns_first_kernel<false>, recs, n, nullptr, t, epoch, seq0, slot_of, ctr, sm_count, st);
 }
 #endif  // FA_HOST_EMUL
+
+// One text for the device and the host emulation (FA_LAUNCH): both kernels loop over tiles / samples grid-stride.
+int launch_feature_fold_counted(int kind, const uint8_t* recs, const unsigned long long* n_dev, uint32_t max_n, const Table& t,
+                                uint64_t epoch, uint64_t seq0, uint32_t* slot_of, Counters* ctr, int sm_count, cudaStream_t st) {
+    if (!max_n) return 0;
+    if (kind == 2) return launch_fold<DropFeat, true>(pktdrop_first_kernel<true>, recs, max_n, n_dev, t, epoch, seq0, slot_of, ctr, sm_count, st);
+    if (kind == 0) return launch_fold<AddFeat, true>(additional_first_kernel<true>, recs, max_n, n_dev, t, epoch, seq0, slot_of, ctr, sm_count, st);
+    return launch_fold<DnsFeat, true>(dns_first_kernel<true>, recs, max_n, n_dev, t, epoch, seq0, slot_of, ctr, sm_count, st);
+}
 
 // ---- eviction: patch the base with the feature effects (feature_patch, kernels.cuh), emit and clear the feature blocks
 // kClear = false: the fa_top_flows / fa_lookup_flows peek, which emits the same rows and leaves the feature lines as

@@ -62,6 +62,9 @@ int launch_full_cut(const uint4* recs, uint32_t n, const Table& table, unsigned 
 // records); slot_of: n u32 scratch
 int launch_feature_fold(int kind, const uint8_t* recs, uint32_t n, const Table& t, uint64_t epoch, uint64_t seq0,
                         uint32_t* slot_of, Counters* ctr, int sm_count, cudaStream_t st);
+// ... of min(*n_dev, max_n) samples, a count that lives in device memory (grids sized from max_n); slot_of: max_n u32
+int launch_feature_fold_counted(int kind, const uint8_t* recs, const unsigned long long* n_dev, uint32_t max_n, const Table& t,
+                                uint64_t epoch, uint64_t seq0, uint32_t* slot_of, Counters* ctr, int sm_count, cudaStream_t st);
 // feature lines per slot, in uint4 (layouts in features.cu): additional_metrics, dns_metrics, pkt_drop_metrics
 constexpr int kAddState = 5;
 constexpr int kDnsState = 8;
@@ -279,6 +282,11 @@ int launch_generate(const GenDeviceParams& g, uint64_t first_index, uint32_t n, 
 struct PeerTargets { uint4* buf[16]; unsigned long long* count[16]; };
 int launch_route_peer(const uint4* recs, const unsigned long long* n_dev, uint32_t max_n, uint32_t n_shards, uint32_t self_shard,
                       const PeerTargets& pt, unsigned long long cap, unsigned long long* overflow, int sm_count, cudaStream_t st);
+// ... the stable variant for K6 samples (kind as launch_feature_fold): pt.buf[o] / pt.count[o] are the caller's segment of
+// owner o's receive buffer (cap samples) and its count word; hist: kMaxShards x ceil(max_n / 256) u32, tot: 16 u64 scratch
+int launch_route_samples(int kind, const uint8_t* samples, const unsigned long long* n_dev, uint32_t max_n, uint32_t n_shards,
+                         const PeerTargets& pt, unsigned long long cap, uint32_t* hist, unsigned long long* tot,
+                         unsigned long long* overflow, int sm_count, cudaStream_t st);
 
 // routing (K3)
 int launch_route(const uint4* recs, uint32_t n, uint32_t n_shards, uint4* out, unsigned long long* counts_dev,

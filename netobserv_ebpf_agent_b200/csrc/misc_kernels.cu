@@ -279,6 +279,51 @@ __global__ void route_scatter_kernel(const uint4* __restrict__ recs, uint32_t n,
 // reservations give, records of one tile keep their order.
 constexpr int kRouteTile = 256;         // records per tile == threads per CTA
 
+// The in-tile partition by owner shared by the routes over peer memory (route_peer_kernel, sample_place_kernel).
+// `o` is the calling thread's owner (0xFF: no record).  Afterwards start[sh] is where owner sh's run begins in the sorted
+// tile (start[n_shards] = the tile's records) and wcount[w][sh] where warp w's records of owner sh begin inside it; the
+// return value is the thread's rank among its warp's records of the same owner.  Stable: runs are owner-major, records
+// keep their tile order inside a run.
+__device__ __forceinline__ uint32_t tile_owner_runs(uint32_t o, uint32_t n_shards, uint32_t (*wcount)[kMaxShards], uint32_t* start) {
+    const uint32_t tid = threadIdx.x, lane = tid & 31u, warp = tid >> 5;
+    const uint32_t same = __match_any_sync(0xFFFFFFFFu, o);                 // lanes of this warp bound for the same owner
+    const uint32_t rank = __popc(same & ((1u << lane) - 1u));
+    if (o != 0xFFu && rank == 0) wcount[warp][o] = __popc(same);
+    __syncthreads();
+    if (tid == 0) {                                                          // runs: owner-major, warps in order inside a run
+        uint32_t acc = 0;
+        for (uint32_t sh = 0; sh < n_shards; sh++) {
+            start[sh] = acc;
+            for (int w = 0; w < kRouteTile / 32; w++) { const uint32_t c = wcount[w][sh]; wcount[w][sh] = acc; acc += c; }
+        }
+        start[n_shards] = acc;
+    }
+    __syncthreads();
+    return rank;
+}
+// ... the sorted position of the calling thread's record
+__device__ __forceinline__ void tile_owner_perm(uint32_t o, uint32_t rank, uint32_t (*wcount)[kMaxShards], uint8_t* perm, uint8_t* owner_of_pos) {
+    if (o != 0xFFu) {
+        const uint32_t pos = wcount[threadIdx.x >> 5][o] + rank;
+        perm[pos] = (uint8_t)threadIdx.x;
+        owner_of_pos[pos] = (uint8_t)o;
+    }
+}
+// ... and the store of the runs: owner sh's run goes to buf[sh] from record cursor[sh] on, W words of T per record, written
+// by consecutive threads in consecutive words (full lines over NVLink).  A record at or past `cap` is not stored: counted.
+template <class T, int W>
+__device__ __forceinline__ void tile_store_runs(uint32_t cnt, const T* tile, const uint8_t* perm, const uint8_t* owner_of_pos,
+                                                const uint32_t* start, const unsigned long long* cursor, const PeerTargets& pt,
+                                                unsigned long long cap, unsigned long long* overflow) {
+    for (uint32_t q = threadIdx.x; q < cnt * W; q += kRouteTile) {
+        const uint32_t pos = q / W, c = q - pos * W;
+        const uint32_t sh = owner_of_pos[pos];
+        const unsigned long long dst = cursor[sh] + (pos - start[sh]);
+        if (dst < cap) reinterpret_cast<T*>(pt.buf[sh])[dst * W + c] = tile[(uint32_t)perm[pos] * W + c];   // peer (or local) memory
+        else if (c == 0) atomicAdd(overflow, 1ull);                          // receive buffer too small: counted, reported at flush
+    }
+}
+
 __global__ void __launch_bounds__(kRouteTile)
 route_peer_kernel(const uint4* __restrict__ recs, const unsigned long long* __restrict__ n_dev, uint32_t max_n,
                   uint32_t n_shards, uint32_t self_shard, PeerTargets pt, unsigned long long cap,
@@ -290,7 +335,7 @@ route_peer_kernel(const uint4* __restrict__ recs, const unsigned long long* __re
     __shared__ uint8_t perm[kRouteTile];                            // sorted position -> record of the tile
     __shared__ uint8_t owner_of_pos[kRouteTile];
     const uint32_t n = n_dev ? (uint32_t)min((unsigned long long)max_n, *n_dev) : max_n;
-    const uint32_t tid = threadIdx.x, lane = tid & 31u, warp = tid >> 5;
+    const uint32_t tid = threadIdx.x;
     // a preceding drain that produced more than its buffer holds has lost records: count them like a receive overflow
     if (n_dev && blockIdx.x == 0 && tid == 0 && *n_dev > (unsigned long long)max_n) atomicAdd(overflow, *n_dev - max_n);
     const uint32_t n_tiles = (n + kRouteTile - 1) / kRouteTile;
@@ -308,46 +353,22 @@ route_peer_kernel(const uint4* __restrict__ recs, const unsigned long long* __re
         }
         if (tid < (kRouteTile / 32) * kMaxShards) (&wcount[0][0])[tid] = 0u;
         __syncthreads();
-        uint32_t o = 0xFFu, rank = 0;
+        uint32_t o = 0xFFu;
         if (tid < cnt) {
             const uint4 k0 = tile[tid * kRecChunks], k1 = tile[tid * kRecChunks + 1], k2 = tile[tid * kRecChunks + 2];
             o = (uint32_t)(owner_hash(key_premix(u64_of(k0.x, k0.y), u64_of(k0.z, k0.w), u64_of(k1.x, k1.y), u64_of(k1.z, k1.w),
                                                  u64_of(k2.x, k2.y))) % n_shards);
         }
-        {
-            const uint32_t same = __match_any_sync(0xFFFFFFFFu, o);          // lanes of this warp bound for the same owner
-            rank = __popc(same & ((1u << lane) - 1u));
-            if (o != 0xFFu && rank == 0) wcount[warp][o] = __popc(same);
-        }
-        __syncthreads();
-        if (tid == 0) {                                                      // runs: owner-major, warps in order inside a run
-            uint32_t acc = 0;
-            for (uint32_t sh = 0; sh < n_shards; sh++) {
-                start[sh] = acc;
-                for (int w = 0; w < kRouteTile / 32; w++) { const uint32_t c = wcount[w][sh]; wcount[w][sh] = acc; acc += c; }
-            }
-            start[n_shards] = acc;
-        }
-        __syncthreads();
+        const uint32_t rank = tile_owner_runs(o, n_shards, wcount, start);
         if (tid < n_shards) {                                                // reserve the run in the owner's receive buffer
             const uint32_t c = start[tid + 1] - start[tid];
             cursor[tid] = c ? atomicAdd_system(pt.count[tid], (unsigned long long)c) : 0ull;
             // overflow[1]: records that leave this GPU (x 144 B = the NVLink payload of the exchange)
             if (tid != self_shard && c) atomicAdd(overflow + 1, (unsigned long long)c);
         }
-        if (o != 0xFFu) {
-            const uint32_t pos = wcount[warp][o] + rank;
-            perm[pos] = (uint8_t)tid;
-            owner_of_pos[pos] = (uint8_t)o;
-        }
+        tile_owner_perm(o, rank, wcount, perm, owner_of_pos);
         __syncthreads();
-        for (uint32_t q = tid; q < cnt * kRecChunks; q += kRouteTile) {
-            const uint32_t pos = q / kRecChunks, c = q - pos * kRecChunks;
-            const uint32_t sh = owner_of_pos[pos];
-            const unsigned long long dst = cursor[sh] + (pos - start[sh]);
-            if (dst < cap) pt.buf[sh][dst * kRecChunks + c] = tile[(uint32_t)perm[pos] * kRecChunks + c];   // peer (or local) memory
-            else if (c == 0) atomicAdd(overflow, 1ull);                       // receive buffer too small: counted, reported at flush
-        }
+        tile_store_runs<uint4, kRecChunks>(cnt, tile, perm, owner_of_pos, start, cursor, pt, cap, overflow);
         __syncthreads();                                                      // the tile and its tables are re-used
     }
     __threadfence_system();                                                   // peer stores visible before the kernel retires
@@ -363,6 +384,118 @@ int launch_route_peer(const uint4* recs, const unsigned long long* n_dev, uint32
     return 1;
 }
 #endif  // FA_HOST_EMUL
+
+// K3 for feature samples (72-byte additional / packet-drop, 104-byte DNS), STABLE: the K6 folds of the owners depend on
+// the order of a flow's samples (first sample adopted whole, last non-zero DNS id / drop cause ...), so a source's samples
+// must reach every owner in the order of the source's slice, not in the order the tiles happen to reserve their runs.
+// Source `self` owns segment `self` of every owner's receive buffer (pt.buf[o] points at it, pt.count[o] at its count
+// word).  Three passes over tiles of 256 samples: count (keys only) -> exclusive scan over (owner, tile) -> place.
+// The place pass sorts each tile by owner in shared memory exactly as route_peer_kernel does, so every owner gets one
+// contiguous run per tile, stored as full lines by consecutive threads, at the offset the scan gave that tile.
+__device__ __forceinline__ uint32_t sample_owner(const uint64_t* k, uint32_t n_shards) {
+    return (uint32_t)(owner_hash(key_premix(k[0], k[1], k[2], k[3], k[4])) % n_shards);
+}
+__device__ __forceinline__ uint32_t sample_count_of(const unsigned long long* n_dev, uint32_t max_n) {
+    return n_dev ? (uint32_t)min((unsigned long long)max_n, *n_dev) : max_n;
+}
+
+// hist[o * n_tiles + tile] = samples of the tile bound for owner o; every tile of the max_n bound gets its row (zeros past
+// the device count), so that the scan needs no count
+template <int kRec>
+__global__ void __launch_bounds__(kRouteTile)
+sample_count_kernel(const uint8_t* __restrict__ samples, const unsigned long long* __restrict__ n_dev, uint32_t max_n,
+                    uint32_t n_shards, uint32_t* __restrict__ hist) {
+    FA_DYN_SMEM(sm);
+    uint32_t* h = reinterpret_cast<uint32_t*>(sm);                  // [kMaxShards]
+    const uint32_t n = sample_count_of(n_dev, max_n), n_tiles = (max_n + kRouteTile - 1) / kRouteTile;
+    const uint32_t tid = threadIdx.x;
+    for (uint32_t tix = blockIdx.x; tix < n_tiles; tix += gridDim.x) {
+        if (tid < kMaxShards) h[tid] = 0u;
+        __syncthreads();
+        const uint32_t i = tix * kRouteTile + tid;
+        uint32_t o = 0xFFu;
+        if (i < n) {
+            const uint64_t* K = reinterpret_cast<const uint64_t*>(samples + (size_t)i * kRec);
+            const uint64_t k[5] = {K[0], K[1], K[2], K[3], K[4]};
+            o = sample_owner(k, n_shards);
+        }
+        const uint32_t same = __match_any_sync(0xFFFFFFFFu, o);
+        if (o != 0xFFu && (same & ((1u << (tid & 31u)) - 1u)) == 0u) atomicAdd(&h[o], (uint32_t)__popc(same));
+        __syncthreads();
+        if (tid < n_shards) hist[tid * n_tiles + tix] = h[tid];
+        __syncthreads();
+    }
+}
+
+// off = route_scan_kernel's exclusive scan of hist (owner-major), tot[o] = owner o's samples.  CTA 0 publishes the
+// segment counts (peer stores); the runs go to pt.buf[o] from (off[o][tile] - off[o][0]) on.
+template <int kRec>
+__global__ void __launch_bounds__(kRouteTile)
+sample_place_kernel(const uint8_t* __restrict__ samples, const unsigned long long* __restrict__ n_dev, uint32_t max_n,
+                    uint32_t n_shards, PeerTargets pt, unsigned long long cap, const uint32_t* __restrict__ off,
+                    const unsigned long long* __restrict__ tot, unsigned long long* overflow) {
+    constexpr int W = kRec / 8;                                      // 8-byte words per sample
+    FA_DYN_SMEM(sm);
+    uint64_t* tile = reinterpret_cast<uint64_t*>(sm);                                            // [kRouteTile * W]
+    unsigned long long* cursor = reinterpret_cast<unsigned long long*>(tile + kRouteTile * W);   // [kMaxShards]
+    uint32_t (*wcount)[kMaxShards] = reinterpret_cast<uint32_t (*)[kMaxShards]>(cursor + kMaxShards);   // [kRouteTile / 32][kMaxShards]
+    uint32_t* start = reinterpret_cast<uint32_t*>(wcount + kRouteTile / 32);                     // [kMaxShards + 1]
+    uint8_t* perm = reinterpret_cast<uint8_t*>(start + kMaxShards + 4);                          // [kRouteTile]
+    uint8_t* owner_of_pos = perm + kRouteTile;                                                   // [kRouteTile]
+    const uint32_t n = sample_count_of(n_dev, max_n), n_tiles = (n + kRouteTile - 1) / kRouteTile, tiles_max = (max_n + kRouteTile - 1) / kRouteTile;
+    const uint32_t tid = threadIdx.x;
+    if (blockIdx.x == 0 && tid < n_shards) *pt.count[tid] = tot[tid];                           // the owner's count word of this segment
+    if (blockIdx.x == 0 && tid == 0 && n_dev && *n_dev > (unsigned long long)max_n) atomicAdd(overflow, *n_dev - max_n);
+    for (uint32_t tix = blockIdx.x; tix < n_tiles; tix += gridDim.x) {
+        const uint32_t first = tix * kRouteTile, cnt = min((uint32_t)kRouteTile, n - first);
+        const uint64_t* G = reinterpret_cast<const uint64_t*>(samples + (size_t)first * kRec);
+        if (cnt == (uint32_t)kRouteTile) {                                   // all loads in flight before the first store
+            uint64_t tmp[W];
+#pragma unroll
+            for (int w = 0; w < W; w++) tmp[w] = G[tid + w * kRouteTile];
+#pragma unroll
+            for (int w = 0; w < W; w++) tile[tid + w * kRouteTile] = tmp[w];
+        } else {
+            for (uint32_t q = tid; q < cnt * W; q += kRouteTile) tile[q] = G[q];
+        }
+        if (tid < (kRouteTile / 32) * kMaxShards) (&wcount[0][0])[tid] = 0u;
+        if (tid < n_shards) cursor[tid] = off[tid * tiles_max + tix] - off[tid * tiles_max];
+        __syncthreads();
+        uint32_t o = 0xFFu;
+        if (tid < cnt) o = sample_owner(tile + tid * W, n_shards);
+        const uint32_t rank = tile_owner_runs(o, n_shards, wcount, start);
+        tile_owner_perm(o, rank, wcount, perm, owner_of_pos);
+        __syncthreads();
+        tile_store_runs<uint64_t, W>(cnt, tile, perm, owner_of_pos, start, cursor, pt, cap, overflow);
+        __syncthreads();                                                      // the tile and its tables are re-used
+    }
+    __threadfence_system();                                                   // peer stores visible before the kernel retires
+}
+
+template <int kRec>
+constexpr size_t sample_place_smem() { return (size_t)kRouteTile * kRec + kMaxShards * 8 + (kRouteTile / 32 + 1) * kMaxShards * 4 + 16 + 2 * kRouteTile; }
+
+// One text for the device and the host emulation (FA_LAUNCH): every kernel loops over tiles grid-stride or runs one CTA.
+// hist: kMaxShards x ceil(max_n / 256) u32, tot: kMaxShards u64 (scratch of the calling engine).
+int launch_route_samples(int kind, const uint8_t* samples, const unsigned long long* n_dev, uint32_t max_n, uint32_t n_shards,
+                         const PeerTargets& pt, unsigned long long cap, uint32_t* hist, unsigned long long* tot,
+                         unsigned long long* overflow, int sm_count, cudaStream_t st) {
+    if (!max_n) return 0;
+    const uint32_t n_tiles = (max_n + kRouteTile - 1) / kRouteTile;
+    const uint32_t grid = std::min<uint32_t>(n_tiles, (uint32_t)sm_count * 5u);
+    if (kind == 1) {
+        FA_LAUNCH(sample_count_kernel<kDnsRecBytes>, grid, kRouteTile, kMaxShards * 4, st, samples, n_dev, max_n, n_shards, hist);
+        FA_LAUNCH(route_scan_kernel, 1, 1024, 0, st, hist, n_tiles, n_shards, tot);
+        FA_LAUNCH(sample_place_kernel<kDnsRecBytes>, grid, kRouteTile, sample_place_smem<kDnsRecBytes>(), st, samples, n_dev, max_n,
+                  n_shards, pt, cap, hist, tot, overflow);
+    } else {                                                          // additional and packet-drop samples: 72 B
+        FA_LAUNCH(sample_count_kernel<kAddRecBytes>, grid, kRouteTile, kMaxShards * 4, st, samples, n_dev, max_n, n_shards, hist);
+        FA_LAUNCH(route_scan_kernel, 1, 1024, 0, st, hist, n_tiles, n_shards, tot);
+        FA_LAUNCH(sample_place_kernel<kAddRecBytes>, grid, kRouteTile, sample_place_smem<kAddRecBytes>(), st, samples, n_dev, max_n,
+                  n_shards, pt, cap, hist, tot, overflow);
+    }
+    return 3;
+}
 
 #ifndef FA_HOST_EMUL
 int launch_route(const uint4* recs, uint32_t n, uint32_t n_shards, uint4* out, unsigned long long* counts_dev,
