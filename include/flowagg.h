@@ -638,7 +638,8 @@ typedef struct fa_iface_name {
                                         pkg/pbflow/proto.go:19-35); without it every record is one Kafka message value
                                         (pkg/exporter/kafka_proto.go:49-60) */
 typedef struct fa_pb_params {
-    uint64_t now_unix_ns;            /* clock() at eviction  (pkg/flow/account.go:103) */
+    uint64_t now_unix_ns;            /* clock() at eviction  (pkg/flow/account.go:103); wall clocks are exact in seconds +
+                                        nanoseconds like time.Time.Add, also past the int64 nanosecond range */
     uint64_t mono_now_ns;            /* monoClock()          (account.go:104) */
     uint8_t  agent_ip[FA_IP_LEN];    /* agent IP in 16-byte form (IPv4: ::ffff:a.b.c.d) */
     uint32_t agent_ip_is_v4;         /* net.IP.To4() != nil */
@@ -655,7 +656,14 @@ typedef struct fa_pb_params {
  * getFlowKey (pkg/exporter/kafka_proto.go:37-47).
  * out_bytes (host or device, out_cap bytes) receives the messages back to back; offsets (n + 1 u64, may be NULL) the
  * start of each; keys_out (n x 32 B, may be NULL) the Kafka keys.  *out_len = bytes needed; FA_E_2BIG if > out_cap
- * (nothing written).  Not produced (no such state in the engine): xlat, quic, network_events_metadata. */
+ * (nothing written).  Not produced (no such state in the engine): xlat, quic, network_events_metadata.
+ * A feature block is used for flow i only where its pointer is given and present[i] has its bit (1 dns, 2 additional,
+ * 4 pkt_drops); present NULL = no block for any flow.
+ * A flow whose dns_name, interface name or UDN is not valid UTF-8 is written as zero bytes (offsets[i] ==
+ * offsets[i + 1]; no Records entry with FA_PB_WRAP_ENTRIES; its key is still written): protobuf-go refuses to marshal
+ * such a `string` field and the Kafka exporter drops the record (pkg/exporter/kafka_proto.go:53-57).  Any other record
+ * is at least a few dozen bytes, so callers skip empty entries.  When every flow is dropped, *out_len is 0 and
+ * out_bytes may be NULL. */
 int fa_pb_encode(fa_engine* e, const void* records, const void* dns, const void* additional, const void* pkt_drops,
                  const uint8_t* present, size_t n, const fa_pb_params* p, void* out_bytes, size_t out_cap, uint64_t* offsets,
                  void* keys_out, size_t* out_len);

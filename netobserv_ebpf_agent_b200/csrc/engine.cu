@@ -1945,7 +1945,7 @@ int fa_pb_encode(fa_engine* e, const void* records, const void* dns, const void*
     CU(cudaStreamSynchronize(e->stream));
     *out_len = (size_t)total;
     if (total > out_cap) return fail(FA_E_2BIG, "fa_pb_encode: %llu bytes needed, capacity %zu", total, out_cap);
-    if (!out_bytes) return fail(FA_E_INVAL, "fa_pb_encode: null out_bytes");
+    if (!out_bytes && total) return fail(FA_E_INVAL, "fa_pb_encode: null out_bytes");   // total 0: every record dropped
     uint8_t* d_out = static_cast<uint8_t*>(out_bytes);
     const bool out_dev = classify(out_bytes) == PTR_DEVICE;
     if (!out_dev) { CU(cudaMalloc(&out_buf.p, total ? total : 16)); d_out = static_cast<uint8_t*>(out_buf.p); }
@@ -1954,7 +1954,7 @@ int fa_pb_encode(fa_engine* e, const void* records, const void* dns, const void*
     if (keys_out && !keys_dev) { CU(cudaMalloc(&keys_buf.p, n * 32)); d_keys = static_cast<uint8_t*>(keys_buf.p); }
     e->st.kernel_launches += fa::launch_pb_write(in, (uint32_t)n, P, e->d_pb_offsets, e->d_pb_sizes, d_out, d_keys, e->stream);
     CU(cudaGetLastError());
-    if (!out_dev) { CU(cudaMemcpyAsync(out_bytes, d_out, total, cudaMemcpyDeviceToHost, e->stream)); e->st.d2h_bytes += total; }
+    if (!out_dev && total) { CU(cudaMemcpyAsync(out_bytes, d_out, total, cudaMemcpyDeviceToHost, e->stream)); e->st.d2h_bytes += total; }
     if (keys_out && !keys_dev) { CU(cudaMemcpyAsync(keys_out, d_keys, n * 32, cudaMemcpyDeviceToHost, e->stream)); e->st.d2h_bytes += n * 32; }
     if (offsets) CU(cudaMemcpyAsync(offsets, e->d_pb_offsets, (n + 1) * 8, cudaMemcpyDefault, e->stream));
     CU(cudaStreamSynchronize(e->stream));

@@ -9,6 +9,9 @@
 // which then leaves with coalesced 16-byte stores; a CTA whose range does not fit writes straight to global memory).
 // Fields are written in field-number order, zero scalars are omitted, sub-messages the reference always allocates
 // (timestamps, data_link, network, transport, agent_ip, time_flow_rtt) are always present — what protobuf-go emits.
+// A record whose dns_name, interface name or UDN is not valid UTF-8 is emitted as zero bytes: protobuf-go refuses to
+// marshal such a `string` field and the Kafka exporter drops the record (pkg/exporter/kafka_proto.go:53-57).  The size
+// pass decides (its size is 0, and a real record is never empty); the write pass reads that size back.
 // Not produced here (the engine has no such state): xlat, quic, network_events_metadata, `interface`, `duplicate`.
 #include "kernels.cuh"
 
@@ -16,8 +19,40 @@ namespace fa {
 
 static_assert(sizeof(PbIface) == 92, "fa_iface_name layout");
 
-struct CountSink { uint32_t n = 0; __device__ __forceinline__ void put(uint8_t) { n++; } };
-struct ByteSink  { uint8_t* p;     __device__ __forceinline__ void put(uint8_t b) { *p++ = b; } };
+// CountSink also checks the string fields (ok); ByteSink only runs on records the CountSink found valid
+struct CountSink { static constexpr bool kCounts = true;  uint32_t n = 0; bool ok = true; __device__ __forceinline__ void put(uint8_t) { n++; } };
+struct ByteSink  { static constexpr bool kCounts = false; uint8_t* p;                      __device__ __forceinline__ void put(uint8_t b) { *p++ = b; } };
+
+// utf8.ValidString: well-formed UTF-8 (Unicode Table 3-7) — no overlong form, surrogate, code point past U+10FFFF,
+// stray continuation byte or truncated sequence
+__device__ __forceinline__ bool utf8_valid(const uint8_t* s, uint32_t len) {
+    uint32_t i = 0;
+    while (i < len) {
+        const uint32_t c = s[i];
+        if (c < 0x80u) { i++; continue; }
+        uint32_t more, lo = 0x80u, hi = 0xBFu;                          // continuation bytes, and the second byte's range
+        if (c >= 0xC2u && c <= 0xDFu) more = 1;
+        else if (c >= 0xE0u && c <= 0xEFu) { more = 2; lo = c == 0xE0u ? 0xA0u : 0x80u; hi = c == 0xEDu ? 0x9Fu : 0xBFu; }
+        else if (c >= 0xF0u && c <= 0xF4u) { more = 3; lo = c == 0xF0u ? 0x90u : 0x80u; hi = c == 0xF4u ? 0x8Fu : 0xBFu; }
+        else return false;
+        if (len - i <= more) return false;
+        if (s[i + 1] < lo || s[i + 1] > hi) return false;
+        for (uint32_t k = 2; k <= more; k++)
+            if ((s[i + k] & 0xC0u) != 0x80u) return false;
+        i += more + 1;
+    }
+    return true;
+}
+// the interface table's strings, 4-byte aligned in their row: an all-ASCII string (the usual one) is checked a word at a
+// time, any other by utf8_valid
+__device__ __forceinline__ bool utf8_valid_row(const char* str, uint32_t len) {
+    const uint8_t* s = reinterpret_cast<const uint8_t*>(str);
+    const uint32_t* w = reinterpret_cast<const uint32_t*>(s);
+    uint32_t high = 0;
+    for (uint32_t k = 0; k < len / 4u; k++) high |= w[k];
+    for (uint32_t k = len & ~3u; k < len; k++) high |= s[k];
+    return (high & 0x80808080u) == 0u || utf8_valid(s, len);
+}
 
 __device__ __forceinline__ uint32_t vlen(uint64_t v) { return v == 0 ? 1u : (uint32_t)(64 - __clzll((long long)v) + 6) / 7u; }
 template <class S> __device__ __forceinline__ void put_varint(S& s, uint64_t v) {
@@ -51,12 +86,16 @@ template <class S> __device__ __forceinline__ void f_ip(S& s, uint32_t field, co
 }
 __device__ __forceinline__ uint32_t f_ip_len(uint32_t field, bool v4) { return vlen((uint64_t)field << 3) + 1u + (v4 ? 5u : 18u); }
 
-// wall clock of a monotonic timestamp: currentTime.Add(-Duration(monoNow - mono)) -> (Unix(), Nanosecond())
+// wall clock of a monotonic timestamp: currentTime.Add(-Duration(monoNow - mono)) -> (Unix(), Nanosecond()).
+// In seconds + nanoseconds, as time.Time.Add does, so that a result outside the int64 nanosecond range (before 1677 or
+// after 2262) stays exact; Go's negation wraps, -Duration(MinInt64) == MinInt64, which is Duration(mono - monoNow).
 __device__ __forceinline__ void wall_of(uint64_t now_unix_ns, uint64_t mono_now, uint64_t mono, int64_t& sec, int32_t& nanos) {
-    const int64_t t = (int64_t)now_unix_ns - (int64_t)(mono_now - mono);
-    int64_t q = t / 1000000000ll, r = t % 1000000000ll;
-    if (r < 0) { r += 1000000000ll; q -= 1; }                       // Go: Unix() floors, Nanosecond() is in [0, 1e9)
-    sec = q; nanos = (int32_t)r;
+    const int64_t d = (int64_t)(mono - mono_now);
+    int64_t s = (int64_t)(now_unix_ns / 1000000000ull) + d / 1000000000ll;
+    int64_t ns = (int64_t)(now_unix_ns % 1000000000ull) + d % 1000000000ll;     // in (-1e9, 2e9)
+    if (ns >= 1000000000ll) { ns -= 1000000000ll; s++; }             // Go: Unix() floors, Nanosecond() is in [0, 1e9)
+    else if (ns < 0) { ns += 1000000000ll; s--; }
+    sec = s; nanos = (int32_t)ns;
 }
 // durationpb.New(d): seconds and nanos truncate towards zero, same sign
 __device__ __forceinline__ void dur_of(uint64_t ns, int64_t& sec, int32_t& nanos) {
@@ -108,6 +147,7 @@ template <class S> __device__ __forceinline__ void f_dup_entry(S& s, const PbPar
     const uint32_t nlen = r ? min((uint32_t)r->name_len, 16u) : 7u;
     const uint8_t* udn = r ? reinterpret_cast<const uint8_t*>(r->udn) : nullptr;
     const uint32_t ulen = r ? min((uint32_t)r->udn_len, 64u) : 0u;
+    if constexpr (S::kCounts) s.ok = s.ok && (!r || (utf8_valid_row(r->name, nlen) && utf8_valid_row(r->udn, ulen)));   // "unknown" is ASCII
     put_tag(s, 26, 2);
     put_varint(s, f_bytes_len(1, nlen) + f_varint_len(2, dir) + f_bytes_len(3, ulen));
     f_bytes(s, 1, name, nlen); f_varint(s, 2, dir); f_bytes(s, 3, udn, ulen);
@@ -160,6 +200,7 @@ __device__ void pb_encode_record(S& s, const uint8_t* rec, const uint8_t* dns, c
         const uint64_t lat = *reinterpret_cast<const uint64_t*>(dns + 16);
         if (lat) { dur_of(lat, sec, nanos); f_secnanos(s, 23, sec, nanos); }
         dname_len = dns_dotted(dns + 31, dname);
+        if constexpr (S::kCounts) s.ok = s.ok && utf8_valid(dname, dname_len);
     }
     dur_of(add ? *reinterpret_cast<const uint64_t*>(add + 16) : 0ull, sec, nanos);   // record.go:123-127; always a message
     f_secnanos(s, 24, sec, nanos);
@@ -193,11 +234,12 @@ __global__ void pb_size_kernel(PbInputs in, uint32_t n, PbParams P, uint32_t* __
         pb_blocks(in, i, dns, add, drop);
         CountSink c;
         pb_encode_record(c, in.recs + (size_t)i * kRecBytes, dns, add, drop, P);
-        sizes[i] = c.n;                                                    // body length; the wrapper is added by pb_total
+        sizes[i] = c.ok ? c.n : 0u;                                        // body length (0: dropped); the wrapper is added by pb_total
     }
 }
 
-__device__ __forceinline__ uint32_t pb_total(uint32_t body, uint32_t wrap) { return wrap ? 1u + vlen(body) + body : body; }
+// a dropped record (body 0) gets no Records entry either
+__device__ __forceinline__ uint32_t pb_total(uint32_t body, uint32_t wrap) { return wrap && body ? 1u + vlen(body) + body : body; }
 
 // exclusive scan of n u32 into u64 offsets (n + 1 entries): per-block sums, one block over the sums, add back
 constexpr int kScanBlock = 1024;
@@ -262,14 +304,16 @@ pb_write_kernel(PbInputs in, uint32_t n, PbParams P, const unsigned long long* _
     const bool staged = total + skew <= (unsigned long long)kPbStage;
     const uint32_t i = first + threadIdx.x;
     if (i < last) {
-        const uint8_t *dns, *add, *drop;
-        pb_blocks(in, i, dns, add, drop);
-        const unsigned long long off = offsets[i] - base;
-        ByteSink w{staged ? stage + skew + off : out + base + off};
-        if (P.wrap) {                                                          // Records.entries = 1, length-delimited
-            w.put(0x0A); put_varint(w, sizes[i]);
+        if (sizes[i]) {                                                        // 0: dropped by the size pass
+            const uint8_t *dns, *add, *drop;
+            pb_blocks(in, i, dns, add, drop);
+            const unsigned long long off = offsets[i] - base;
+            ByteSink w{staged ? stage + skew + off : out + base + off};
+            if (P.wrap) {                                                      // Records.entries = 1, length-delimited
+                w.put(0x0A); put_varint(w, sizes[i]);
+            }
+            pb_encode_record(w, in.recs + (size_t)i * kRecBytes, dns, add, drop, P);
         }
-        pb_encode_record(w, in.recs + (size_t)i * kRecBytes, dns, add, drop, P);
         if (keys_out) {                                                        // getFlowKey: the smaller address first
             const uint8_t* id = in.recs + (size_t)i * kRecBytes;
             int cmp = 0;
